@@ -2,6 +2,7 @@
 """bench.py -- MTTKRP nnz*R/sec per mode on synthetic sparse tensors (BASELINE.json).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+                    [--dump-outputs DIR]
 
 A "step" is one MTTKRP sweep: one MTTKRP per mode of the tensor (the hot path of
 one CPD-ALS iteration).  value = nnz_total * R * nmodes / step time = the mean
@@ -37,7 +38,13 @@ Also in the JSON line:
                    (SPLATT_B200_NGPUS=N), run by rank 0 while the other ranks idle.
 
 `--impl reference` times the reference's own OpenMP mttkrp_csf (oracle/_ref,
-compiled unmodified from /root/reference) on the host cores on the same workload.
+compiled unmodified from the reference sources by oracle/build_ref.sh) on the host cores on
+the same workload.
+
+`--dump-outputs DIR` writes, after the timed steps, what the headline sweep computed in its
+last timed step: DIR/mttkrp_mode<m>.npy, the float64 dims[m] x R output of every mode (the
+factor a caller receives; summed over ranks at N > 1), 7.7 MB in all.  Inputs are seeded, so
+two builds run with the same arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -60,7 +67,7 @@ NNZ_PER_GPU = 10_000_000
 RANK = 32
 NMODES = 3
 SEED = 1
-FALLBACK_HBM_GBS = 6650.0
+FALLBACK_HBM_GBS = 3350.0          # H100 SXM data sheet (HBM3)
 
 NAMED = {
     "4": {"name": "BASELINE.json configs[3]: synthetic uniform 3-mode 100000^3, 100M nnz, rank 32",
@@ -77,7 +84,7 @@ def log(*a):
 
 # --------------------------------------------------------------------------- clocks
 class ClockSampler:
-    """nvidia-smi sampling during the timed region (B200_PROFILING.md clocks line)."""
+    """nvidia-smi sampling of SM clock, power and throttle reasons during the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,"
          "clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -171,18 +178,7 @@ def hbm_peak():
             return float(json.loads(p.read_text())["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
         except Exception:
             pass
-    return FALLBACK_HBM_GBS, "fallback (B200_PROFILING.md)"
-
-
-def ncu_traffic():
-    """DRAM bytes per launch of the dominant kernel from the committed ncu capture."""
-    p = ROOT / "profiles" / "traffic.json"
-    if p.exists():
-        try:
-            return json.loads(p.read_text()).get("dram_bytes_per_launch")
-        except Exception:
-            return None
-    return None
+    return FALLBACK_HBM_GBS, "fallback (H100 SXM data sheet)"
 
 
 def rel_fro(a, b):
@@ -325,7 +321,7 @@ def workload_config(n_gpus):
 def gather_probe_gbs(dev):
     """Measured rate of the access pattern that bounds the kernel at the KERNEL's own shape
     (24 warps/SM, 8 rows in flight): random whole-row fp64 gathers (RANK columns) from a
-    DIM-row matrix, nothing else.  The ceiling over all shapes is in profiles/ (probe sweep)."""
+    DIM-row matrix, nothing else."""
     import ctypes as C
     import torch
     from splatt_b200 import _abi as A
@@ -355,14 +351,6 @@ def gather_probe_gbs(dev):
         ts.append(e0.elapsed_time(e1))
     ms = float(np.median(ts))
     return n * RANK * 8 / (ms * 1e-3) / 1e9, ms
-
-
-def probe_sweep_best():
-    p = ROOT / "profiles" / "r02_probe_sweep_R32.json"
-    try:
-        return json.loads(p.read_text())["best"]
-    except Exception:
-        return None
 
 
 def cpd_iteration_times(S, csf, ind, vals, mats_h, ref_threads=None):
@@ -512,8 +500,9 @@ class Workload:
         torch.cuda.synchronize()
         return [c.cpu().numpy() for c in cap]
 
-    def timed(self, flush, steps, warmup):
-        """W warm-up steps, then K steps back to back; returns per-step ms, per-mode ms lists."""
+    def timed(self, flush, steps, warmup, capture=None):
+        """W warm-up steps, then K steps back to back; returns per-step ms, per-mode ms lists.
+        capture: a list of nmodes entries that receives the last step's summed outputs."""
         import torch
         for _ in range(warmup):
             flush.zero_()
@@ -529,9 +518,13 @@ class Workload:
         for k in range(steps):
             flush.zero_()
             ev[k][0].record()
-            self.sweep(kev[k])
+            # the fused exchange re-zeroes its buffer right after each mode: the last step's
+            # result must be copied out inside the step; otherwise it stays in self.outs
+            self.sweep(kev[k], capture if k == steps - 1 and self.fx is not None else None)
             ev[k][1].record()
         self.ctx.barrier()
+        if capture is not None and self.fx is None:
+            capture[:] = [o.clone() for o in self.outs]
         wall = time.time() - w0
         self.launches = S.launch_count() - l0
         step_ms = [a.elapsed_time(b) for a, b in ev]
@@ -602,8 +595,8 @@ def run_named(ctx, key, args, flush):
     del ind, vals
     torch.cuda.empty_cache()
     ours = wl.outputs_host()
-    steps = max(5, min(args.steps, 10))
-    step_ms, mode_ms, _ = wl.timed(flush, steps, max(args.warmup, 3))
+    steps = args.steps
+    step_ms, mode_ms, _ = wl.timed(flush, steps, args.warmup)
     ms_per_step = ctx.max_over_ranks(float(np.sum(step_ms))) / steps
     per_mode = [ctx.max_over_ranks(float(np.mean(mode_ms[m]))) for m in range(wl.N)]
     wl.keep_busy(flush, 0.3)
@@ -698,8 +691,15 @@ def run_ours(args):
     ind, vals = make_coo_gpu(nnz_total, dev)
     wl = Workload(ctx, dims, ind, vals, RANK, args.nccl_exchange, SEED)
     ours_host = wl.outputs_host()          # also warms the GPU up before the W warm-up steps
-    step_ms, kern_ms, wall_s = wl.timed(flush, args.steps, max(args.warmup, 3))
+    last = [None] * NMODES if args.dump_outputs else None
+    step_ms, kern_ms, wall_s = wl.timed(flush, args.steps, args.warmup, last)
     launches = wl.launches
+    if last is not None and rank == 0:
+        out_dir = Path(args.dump_outputs)
+        out_dir.mkdir(parents=True, exist_ok=True)
+        for m, o in enumerate(last):
+            np.save(out_dir / f"mttkrp_mode{m}.npy", o.cpu().numpy().astype(np.float64))
+        del last
     ms_per_step = ctx.max_over_ranks(float(np.sum(step_ms))) / args.steps
     worst_step = ctx.max_over_ranks(float(np.max(step_ms)))
     best_step = ctx.max_over_ranks(float(np.min(step_ms)))
@@ -799,15 +799,14 @@ def run_ours(args):
                 peak_gbs, probe_ms = gather_probe_gbs(dev)
                 gb = info[0]["nfibs"][-1] * RANK * 8 + info[0]["nfibs"][-2] * RANK * 8
                 gather_numbers = {"achieved_GBps": gb / (k_ms * 1e-3) / 1e9,
-                                  "probe_same_shape_GBps": peak_gbs, "probe_ms": probe_ms,
-                                  "probe_sweep_best": probe_sweep_best()}
+                                  "probe_same_shape_GBps": peak_gbs, "probe_ms": probe_ms}
         except Exception as e:  # pragma: no cover
             gather_numbers = {"probe_error": str(e)}
         achieved = alg / (k_ms * 1e-3) / 1e9
         roof = {"bound": "hbm", "kernel": "mttkrp_stream_kernel<3,16,root> (mode 0)",
                 "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
                 "peak_source": how, "alg_bytes_per_launch": alg,
-                "launch_ms": k_ms, "traffic": ncu_traffic(),
+                "launch_ms": k_ms,
                 "per_mode_ms": [float(np.mean(k)) for k in kern_ms],
                 "gather_path": dict(gather_numbers, **{
                     "bytes_per_launch": int(info[0]["nfibs"][-1] * RANK * 8 +
@@ -873,7 +872,7 @@ def run_ours(args):
             except Exception as e:  # pragma: no cover
                 cpd = dict(cpd_multi or {}, error=f"{type(e).__name__}: {e}")
         line = {"metric": "MTTKRP nnz*R/sec per mode", "value": value, "unit": "nnz*R/s",
-                "n_gpus": n_gpus, "steps": args.steps, "warmup": max(args.warmup, 3),
+                "n_gpus": n_gpus, "steps": args.steps, "warmup": args.warmup,
                 "ms_per_step": ms_per_step, "higher_is_better": True, "scaling": "weak",
                 "vs_baseline": None, "dtype": "f64", "data": "synthetic",
                 "config": workload_config(n_gpus),      # identical in both arms
@@ -901,9 +900,11 @@ def run_ours(args):
         sys.stdout.flush()
         sys.stderr.flush()
         print(json.dumps(line), flush=True)
-        # the JSON line must be the LAST line on stdout: with NCCL_DEBUG=INFO the library
-        # prints from its exit handlers ("Closing env plugin ...") -- leave without running them
-        os._exit(0)
+        if world > 1:
+            # the JSON line must be the LAST line on stdout: with NCCL_DEBUG=INFO the library
+            # prints from its exit handlers ("Closing env plugin ...") -- leave without running
+            # them.  One GPU has no process group and no NCCL: the process ends normally.
+            os._exit(0)
     return 0
 
 
@@ -916,10 +917,14 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--nccl-exchange", action="store_true",
                     help="N>1: use kernel + NCCL all-reduce instead of the fused multicast exchange")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's outputs as DIR/mttkrp_mode<m>.npy")
     ap.add_argument("--named", default="4,5",
                     help="named multi-GPU configs to run after the headline workload "
                          "(BASELINE.json configs[3] = 4, configs[4] = 5; '' = none)")
     args = ap.parse_args()
+    if args.steps < 1 or args.warmup < 0:
+        ap.error("--steps must be >= 1 and --warmup >= 0")
     if args.impl == "reference":
         return run_reference(args)
     return run_ours(args)

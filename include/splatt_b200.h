@@ -1,5 +1,5 @@
 /*
- * splatt_b200.h -- C ABI of libsplatt_b200.so, the B200-native MTTKRP engine
+ * splatt_b200.h -- C ABI of libsplatt_b200.so, the Hopper (H100, sm_90a) MTTKRP engine
  * that drops in behind SPLATT's MTTKRP / CPD-ALS entry points.
  *
  * Two groups of symbols:
@@ -11,8 +11,7 @@
  *      ShadenSmith/splatt tree).  The struct layouts below are written to be
  *      binary compatible with the reference's default configuration
  *      (idx = uint64, val = double, SPLATT_MAX_NMODES = 8); tests/test_abi.py
- *      proves the offsets against the reference headers whenever the reference
- *      tree is present.
+ *      proves the offsets against ones recorded from the reference headers.
  *
  *  (2) ENGINE symbols (prefix splatt_b200_).  The device-resident interface:
  *      tensors live in HBM as per-mode "fiber streams", factor matrices and
@@ -506,7 +505,7 @@ uint64_t splatt_b200_build_count(void);
  * Call this before freeing a CSF whose mirror should release its HBM now. */
 void splatt_b200_cache_clear(void);
 
-/* Library / build identification, e.g. "splatt_b200 0.1 sm_100a". */
+/* Library / build identification, e.g. "splatt_b200 0.1 (sm_90a fiber-stream MTTKRP)". */
 char const * splatt_b200_version(void);
 
 #ifdef __cplusplus

@@ -1,7 +1,7 @@
 """TEST INFRASTRUCTURE ONLY.
 
 oracle/ holds the checkers for the MTTKRP / CPD-ALS hot path:
-  * oracle/_ref/      the UNMODIFIED reference, compiled from /root/reference by
+  * oracle/_ref/      the UNMODIFIED reference, compiled from the reference sources by
                       oracle/build_ref.sh (+ ref_driver.c, a flat ctypes facade).
                       `oracle.ref` wraps it.
   * oracle/restate.c  a plain-C restatement of the reference's algorithms for this

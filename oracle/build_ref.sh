@@ -1,6 +1,7 @@
 #!/usr/bin/env bash
 # TEST INFRASTRUCTURE ONLY -- builds the *unmodified* reference (ShadenSmith/splatt)
-# from the sources where they lie under /root/reference into oracle/_ref/.
+# from its sources (SPLATT_REFERENCE names the tree) into oracle/_ref/; without
+# the sources it keeps whatever oracle/_ref/ holds and exits 0.
 # Nothing under oracle/ is ever linked, imported or executed by the product
 # (splatt_b200/, libsplatt_b200.so); only tests/, __graft_entry__.smoke() and
 # bench.py's cpu_baseline / --impl reference legs use it, as the checker.
@@ -10,10 +11,10 @@
 # (cmake/types.cmake:48-49).  We generate that one header into oracle/_ref/gen/
 # with the default widths (idx 64, val 64, blas-int 32; cmake/types.cmake:3-4)
 # and compile src/*.c directly with the reference's release flags
-# (cmake/flags.cmake:5-16) minus -march=native (the GPU box host CPU may differ
+# (cmake/flags.cmake:5-16) minus -march=native (the GPU host's CPU may differ
 # from the build container; x86-64-v3 = AVX2+FMA is used instead).
 #
-# Outputs (git-ignored, shipped to the GPU box by gpurun):
+# Outputs (git-ignored):
 #   oracle/_ref/libsplatt_ref.so   reference library (all of src/*.c, OpenMP) + ref_driver.c
 #   oracle/_ref/splatt             reference CLI (src/cmds/*.c), BASELINE config #1
 #   oracle/_ref/splatt_gpu         the same CLI linked against libsplatt_b200.so for the
@@ -75,8 +76,11 @@ gcc -fopenmp -o "$OUT/splatt" "${cmdobjs[@]}" "${objs[@]}" \
 # symbols of src/mttkrp.c renamed out of the way (objcopy, no source edits) so that
 # cpd.c / bench.c / the tests resolve splatt_mttkrp_csf, splatt_mttkrp_alloc_ws,
 # splatt_mttkrp_free_ws and splatt_mttkrp from libsplatt_b200.so (INTEGRATION.md,
-# option A).  `splatt_gpu cpd ...` = reference host code + B200 MTTKRP.
+# option A).  `splatt_gpu cpd ...` = reference host code + GPU MTTKRP.
 B200LIB="$HERE/../splatt_b200/libsplatt_b200.so"
+# linked by name, not by path: the binaries then find the library through the $ORIGIN rpath
+# wherever the tree is moved after the build
+B200LINK=(-L"$HERE/../splatt_b200" -lsplatt_b200)
 if [ -f "$B200LIB" ]; then
   objcopy --redefine-sym splatt_mttkrp_csf=splatt_mttkrp_csf_cpu \
           --redefine-sym splatt_mttkrp=splatt_mttkrp_cpu \
@@ -87,7 +91,7 @@ if [ -f "$B200LIB" ]; then
   for o in "${objs[@]}"; do
     case "$o" in */mttkrp.o) gpuobjs+=("$OUT/obj/mttkrp_cpu.o");; *) gpuobjs+=("$o");; esac
   done
-  gcc -fopenmp -o "$OUT/splatt_gpu" "${cmdobjs[@]}" "${gpuobjs[@]}" "$B200LIB" \
+  gcc -fopenmp -o "$OUT/splatt_gpu" "${cmdobjs[@]}" "${gpuobjs[@]}" "${B200LINK[@]}" \
       "$BLASLIB" -Wl,--disable-new-dtags,-rpath,"$BLASDIR" -Wl,-rpath,'$ORIGIN/../../splatt_b200' -lm -lrt
 fi
 # The reference's OWN MTTKRP unit tests (tests/mttkrp_test.c: every fixture x every mode x
@@ -107,7 +111,7 @@ done
 gcc -fopenmp -o "$OUT/reftest_mttkrp_cpu" "${tobjs[@]}" "${objs[@]}" \
     "$BLASLIB" -Wl,--disable-new-dtags,-rpath,"$BLASDIR" -lm -lrt
 if [ -f "$B200LIB" ]; then
-  gcc -fopenmp -o "$OUT/reftest_mttkrp_gpu" "${tobjs[@]}" "${gpuobjs[@]}" "$B200LIB" \
+  gcc -fopenmp -o "$OUT/reftest_mttkrp_gpu" "${tobjs[@]}" "${gpuobjs[@]}" "${B200LINK[@]}" \
       "$BLASLIB" -Wl,--disable-new-dtags,-rpath,"$BLASDIR" -Wl,-rpath,'$ORIGIN/../../splatt_b200' -lm -lrt
 fi
 rm -rf "$OUT/obj"

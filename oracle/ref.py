@@ -27,7 +27,7 @@ def load() -> C.CDLL:
     if _lib is not None:
         return _lib
     if not LIB_PATH.exists():
-        raise RuntimeError(f"{LIB_PATH} missing; run oracle/build_ref.sh where /root/reference exists")
+        raise RuntimeError(f"{LIB_PATH} missing; run oracle/build_ref.sh where the reference sources exist")
     lib = C.CDLL(str(LIB_PATH), mode=os.RTLD_LOCAL)
     u64p = C.POINTER(C.c_uint64)
     u64pp = C.POINTER(u64p)

@@ -2,7 +2,7 @@
  * ref_driver.c -- TEST INFRASTRUCTURE ONLY (never linked into the product).
  *
  * A flat, ctypes-friendly C interface over the UNMODIFIED reference library
- * (oracle/_ref/libsplatt_ref.so, built from /root/reference by build_ref.sh).
+ * (oracle/_ref/libsplatt_ref.so, built from the reference sources by build_ref.sh).
  * Compiled against the reference's own headers, so every struct and call here
  * is the reference's; this file contributes no arithmetic of its own.
  *

@@ -1,6 +1,6 @@
-"""splatt_b200 -- a B200-native MTTKRP engine behind SPLATT's C API.
+"""splatt_b200 -- an H100-native MTTKRP engine behind SPLATT's C API.
 
-The product is splatt_b200/libsplatt_b200.so (hand-written sm_100a CUDA, C ABI in
+The product is splatt_b200/libsplatt_b200.so (hand-written sm_90a CUDA, C ABI in
 include/splatt_b200.h).  This package is the thin Python host layer over it.
 """
 from . import _abi  # noqa: F401

@@ -1,9 +1,9 @@
-"""In-tree build of libsplatt_b200.so (nvcc, sm_100a only).
+"""In-tree build of libsplatt_b200.so (nvcc, sm_90a only).
 
 `python -m splatt_b200.build` or `splatt_b200.build.build()`.  Objects are
 compiled in parallel (one nvcc per translation unit; the kernel templates are
 instantiated once per mode count) and linked into splatt_b200/libsplatt_b200.so,
-which ships to the GPU box with the repo snapshot.
+next to the package sources.
 """
 from __future__ import annotations
 
@@ -21,7 +21,7 @@ OUT = HERE / "libsplatt_b200.so"
 OBJ = HERE / "_obj"
 
 NVCC = os.environ.get("NVCC") or shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC,-fopenmp,-O3",
           "-Xcudafe", "--diag_suppress=177"]
 

@@ -194,7 +194,7 @@ int build_tensor(int N, const uint64_t * dims, const DevCoo & dc,
   T->shard_count = bo.shard_count > 1 ? bo.shard_count : 1;
   if (cudaGetDevice(&T->device) != cudaSuccess) { delete T; return SPLATT_ERROR_BADINPUT; }
   T->streams.resize(stream_perms.size());
-  int num_sms = 148;
+  int num_sms = 132;
   cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, T->device);
   for (size_t i = 0; i < stream_perms.size(); ++i) {
     // Leaf-tile re-ordering policy.  Worth it only when a leaf row is re-used several
@@ -655,6 +655,6 @@ void splatt_b200_shard_range(uint64_t nnz, int rank, int count_shards, uint64_t 
 uint64_t splatt_b200_launch_count(void) { return g_spb200_launches; }
 uint64_t splatt_b200_build_count(void) { return g_spb200_builds; }
 
-char const * splatt_b200_version(void) { return "splatt_b200 0.1 (sm_100a fiber-stream MTTKRP)"; }
+char const * splatt_b200_version(void) { return "splatt_b200 0.1 (sm_90a fiber-stream MTTKRP)"; }
 
 }  // extern "C"

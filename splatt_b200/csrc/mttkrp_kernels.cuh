@@ -1,4 +1,4 @@
-// sm_100a MTTKRP kernels over fiber streams (see common.h for the layout).
+// sm_90a MTTKRP kernels over fiber streams (see common.h for the layout).
 //
 // Replaces the reference's CPU kernels (src/mttkrp.c):
 //   KIND_ROOT  p_csf_mttkrp_root3_* :390-541, p_csf_mttkrp_root_* :668-799

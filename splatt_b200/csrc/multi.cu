@@ -5,7 +5,7 @@
 // node: the tensor is partitioned, every device computes the MTTKRP of its share, the
 // output factor is summed over devices once per mode, the dense tail is row-partitioned
 // over the devices (single-valued factors; see splatt_b200_multi_cpd_als).
-// Differences that make it B200-native:
+// Differences that make it native to an NVSwitch box of H100s:
 //   * partition = equal-nnz contiguous chunk ranges of every fiber stream (built once on
 //     the first device, the shares are cut out and moved device-to-device);
 //   * exchange  = inside the MTTKRP kernel: every finished output row goes into ALL devices'
@@ -457,7 +457,7 @@ int multi_mttkrp_enqueue(splatt_b200_multi * h, int mode) {
       if (p != i) MCK(cudaStreamWaitEvent(s.stream, h->d[p].ev_k, 0));
     const unsigned long long e0 = I * i / k * half, e1 = I * (i + 1) / k * half;
     if (e1 > e0) {
-      const unsigned blocks = (unsigned)std::min<unsigned long long>((e1 - e0 + 255) / 256, 148ull * 8);
+      const unsigned blocks = (unsigned)std::min<unsigned long long>((e1 - e0 + 255) / 256, 132ull * 8);
       k_peer_reduce<<<blocks, 256, 0, s.stream>>>(a, e0, e1);
       spb200_count_launches(1);
       MCK(cudaGetLastError());

@@ -10,7 +10,7 @@ if str(ROOT) not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
 
 
 @pytest.fixture(scope="session")
@@ -24,6 +24,6 @@ def refmod():
     """The compiled, unmodified reference (oracle/_ref).  Skips when it was not built."""
     from oracle import ref
     if not ref.available():
-        pytest.skip("oracle/_ref not built (needs /root/reference at build time)")
+        pytest.skip("oracle/_ref not built (needs the reference sources at build time)")
     ref.load()
     return ref

@@ -8,6 +8,7 @@ import numpy as np
 import pytest
 
 from splatt_b200 import _abi as A
+from tests import recorded
 
 ROOT = Path(__file__).resolve().parent.parent
 
@@ -34,10 +35,11 @@ def test_version_and_default_opts(lib):
     assert o[A.OPTION_VERBOSITY] == A.VERBOSITY_LOW and o[A.OPTION_NTHREADS] >= 1
 
 
-def test_struct_layouts_match_reference_headers(refmod):
+def test_struct_layouts_match_reference_headers():
     """Offsets computed by the C compiler from the reference's own headers
-    (oracle/ref_driver.c:refdrv_abi) vs the ctypes mirror of include/splatt_b200.h."""
-    f = iter(refmod.abi_facts())
+    (oracle/ref_driver.c:refdrv_abi, recorded in tests/golden/reference.npz) vs the ctypes
+    mirror of include/splatt_b200.h."""
+    f = iter(recorded.load()["abi_facts"].tolist())
 
     def nxt():
         return next(f)
@@ -65,7 +67,7 @@ def test_struct_layouts_match_reference_headers(refmod):
     assert [nxt() for _ in range(13)] == list(range(13))     # option enum order
 
 
-def test_header_struct_layout_compiles_to_the_same_offsets(tmp_path, refmod):
+def test_header_struct_layout_compiles_to_the_same_offsets(tmp_path):
     """Compile include/splatt_b200.h with gcc and compare sizeof/offsetof to the reference."""
     import subprocess
     src = tmp_path / "abi.c"
@@ -83,7 +85,7 @@ int main(void){
     subprocess.run(["gcc", "-std=c99", f"-I{ROOT / 'include'}", str(src), "-o", str(exe)], check=True)
     got = [int(x) for x in subprocess.run([str(exe)], capture_output=True, text=True,
                                           check=True).stdout.split()]
-    facts = refmod.abi_facts()
+    facts = recorded.load()["abi_facts"].tolist()
     assert got[:5] == [facts[3], facts[8], facts[19], facts[26], facts[35]]
     assert got[5:] == [A.SplattCsf.which_tile.offset, A.SplattCsf.ntiles.offset,
                        A.SplattCsf.pt.offset, A.MttkrpWs.privatize_buffer.offset]

@@ -20,6 +20,10 @@ def _write_tns(path, ind, vals):
             f.write(f" {float(vals[n])!r}\n")
 
 
+def cli_fits(stdout):
+    return [float(x) for x in re.findall(r"fit = ([0-9.]+)", stdout)]
+
+
 @pytest.mark.skipif(not ref.CLI_PATH.exists(), reason="oracle/_ref/splatt not built")
 def test_reference_cli_cpd_on_med_fixture(tmp_path):
     z = np.load(GOLD / "med.npz")
@@ -29,10 +33,11 @@ def test_reference_cli_cpd_on_med_fixture(tmp_path):
                         "--nowrite", "-i", "5"], capture_output=True, text=True, timeout=300)
     assert r.returncode == 0, r.stderr
     out = r.stdout
-    assert "DIMS=2425x10816x29567" in out and "NNZ=100000" in out
-    fits = [float(x) for x in re.findall(r"fit = ([0-9.]+)", out)]
+    dims = "x".join(str(int(z["ind"][m].max()) + 1) for m in range(z["ind"].shape[0]))
+    assert f"DIMS={dims}" in out and f"NNZ={len(z['vals'])}" in out
+    fits = cli_fits(out)
     assert len(fits) == 5
-    assert abs(fits[-1] - 0.00087) < 2e-5          # SURVEY.md 8(c): fit 0.00087 after 5 its
+    assert abs(fits[-1] - z["cli_fit_r16_i5"][0]) < 2e-5       # recorded by tests/golden/make_golden.py
     assert "Final fit" in out
 
 
@@ -60,7 +65,7 @@ def test_reference_cli_linked_against_libsplatt_b200(tmp_path, name, rank, gpus)
     libsplatt_b200.so (objcopy rename, INTEGRATION.md option A).  Same seed => the GPU-backed run
     prints the same fit trajectory as the pure-CPU run.  `gpus`: one GPU; the single-process
     multi-GPU engine on a device list that names GPU 0 twice (SPLATT_B200_DEVICES=0,0); and
-    SPLATT_B200_NGPUS=2 on two real GPUs (gpurun --gpus 2) -- the reference's C host driving
+    SPLATT_B200_NGPUS=2 on two real GPUs -- the reference's C host driving
     several GPUs through the unchanged C API (the shape of src/mpi/mpi_cpd.c:627-804)."""
     import torch
     env = dict(os.environ)
@@ -68,7 +73,7 @@ def test_reference_cli_linked_against_libsplatt_b200(tmp_path, name, rank, gpus)
         env["SPLATT_B200_DEVICES"] = "0,0"
     elif gpus == "ngpus-2":
         if torch.cuda.device_count() < 2:
-            pytest.skip("needs >= 2 GPUs (gpurun --gpus 2)")
+            pytest.skip("needs >= 2 GPUs")
         env["SPLATT_B200_NGPUS"] = "2"
     z = np.load(GOLD / f"{name}.npz")
     tns = tmp_path / f"{name}.tns"
@@ -117,6 +122,6 @@ def test_reference_bench_harness_on_gpu(tmp_path, name):
         assert "** CSF **" in r.stdout
         outs[tag] = [np.loadtxt(wd / f"csf_mode{m + 1}.mat") for m in range(len(z["dims"]))]
     for m, (a, b) in enumerate(zip(outs["cpu"], outs["gpu"])):
-        assert a.shape == b.shape == (int(z["dims"][m]), 8)
+        assert a.shape == b.shape == (int(z["ind"][m].max()) + 1, 8)     # dims as tt_read finds them
         # the dump keeps 9 significant digits
         assert np.allclose(a, b, rtol=1e-7, atol=1e-7), m

@@ -1,39 +1,29 @@
 """GPU parity: the CUDA path, called through the C ABI, against the reference.
 
-Gold is the reference's own gold (tests/mttkrp_test.c:66): mttkrp_stream on COO,
-computed by the unmodified reference in oracle/_ref.  The north-star bar is
-1e-6 relative Frobenius; fp64 with a different summation order lands ~1e-15, so
-the tests assert 1e-11 (and the reference's own abs 1e-10 scaled by magnitude).
+Gold is the reference's own gold (tests/mttkrp_test.c:66), mttkrp_stream on COO, as
+oracle/restate.c restates it; tests/test_oracle.py pins that restatement (and its CPD-ALS)
+to output recorded from the compiled reference.  CSFs in the reference's layout come from
+splatt_b200_csf_alloc, whose arrays test_csf_alloc_matches_reference pins to the ones the
+reference's csf_alloc builds.  The north-star bar is 1e-6 relative Frobenius; fp64 with a
+different summation order lands ~1e-15, so the tests assert 1e-11 (and the reference's own
+abs 1e-10 scaled by magnitude).
 """
 import os
-import zlib
 
 import numpy as np
 import pytest
 
-from tests.util import cover_all_slices, factor_mats, random_coo, rel_fro
+from oracle import restate
+from tests import recorded
+from tests.util import (PARITY_TENSORS, cover_all_slices, factor_mats, mttkrp_gold, parity_tensor,
+                        random_coo, rel_fro)
 
 pytestmark = pytest.mark.gpu
 
 TOL = 1e-11
 
-TENSORS = {
-    "t2_matrix": ((300, 500), 9000),
-    "t3_small": ((13, 7, 11), 150),
-    "t3_mid": ((300, 200, 400), 20000),
-    "t3_long_fibers": ((50, 40, 3000), 30000),
-    "t3_skew": ((2000, 1500, 60), 40000),
-    "t4": ((40, 30, 50, 20), 15000),
-    "t5": ((12, 15, 10, 20, 9), 8000),
-    "t6": ((6, 7, 5, 8, 9, 4), 4000),
-    "t8": ((4, 3, 5, 4, 3, 6, 2, 5), 3000),
-}
-
-
-def _tensor(name):
-    dims, nnz = TENSORS[name]
-    skew = [1.0, 1.0, 0] if name == "t3_skew" else None
-    return random_coo(dims, nnz, seed=zlib.crc32(name.encode()) % 1000, skew=skew)   # stable seed
+TENSORS = [n for n in PARITY_TENSORS if n != "t3_tiny"]
+_tensor = parity_tensor
 
 
 @pytest.fixture(scope="module")
@@ -42,26 +32,21 @@ def S():
     return splatt_b200
 
 
-def _gold(refmod, dims, inds, vals, mats):
-    tt = refmod.RefTensor.from_coo(dims, inds, vals)
-    return tt, [tt.mttkrp_stream(mats, m) for m in range(len(dims))]
-
-
 @pytest.mark.parametrize("name", list(TENSORS))
 @pytest.mark.parametrize("R", [3, 16, 32])
 @pytest.mark.parametrize("layout", ["allroot", "asgiven"])
-def test_dropin_mttkrp_on_reference_csf(S, refmod, name, R, layout, monkeypatch):
-    """splatt_mttkrp (ours) on CSFs built by the reference's csf_alloc, every mode,
-    every allocation policy -- the drop-in scenario."""
+def test_dropin_mttkrp_on_reference_csf(S, name, R, layout, monkeypatch):
+    """splatt_mttkrp (ours) on CSFs laid out as the reference's csf_alloc lays them out,
+    every mode, every allocation policy -- the drop-in scenario."""
     monkeypatch.setenv("SPLATT_B200_LAYOUT", layout)
     dims, inds, vals = _tensor(name)
     mats = factor_mats(dims, R)
-    tt, gold = _gold(refmod, dims, inds, vals, mats)
+    gold = mttkrp_gold(dims, inds, vals, mats)
     for alloc in (0, 1, 2):
-        o = refmod.default_opts()
+        o = S.default_opts()
         o[0] = 1
         o[6] = alloc
-        csf = refmod.RefCsf(tt, o)
+        csf = S.csf_alloc(dims, inds, vals, o)
         for m in range(len(dims)):
             out = S.mttkrp(m, R, csf.ptr, mats, o)
             assert rel_fro(out, gold[m]) < TOL, (name, R, layout, alloc, m)
@@ -69,13 +54,13 @@ def test_dropin_mttkrp_on_reference_csf(S, refmod, name, R, layout, monkeypatch)
 
 
 @pytest.mark.parametrize("R", [1, 2, 5, 10, 48, 64, 70, 130])
-def test_ranks(S, refmod, R):
+def test_ranks(S, R):
     dims, inds, vals = _tensor("t3_mid")
     mats = factor_mats(dims, R)
-    tt, gold = _gold(refmod, dims, inds, vals, mats)
-    o = refmod.default_opts()
+    gold = mttkrp_gold(dims, inds, vals, mats)
+    o = S.default_opts()
     o[0] = 1
-    csf = refmod.RefCsf(tt, o)
+    csf = S.csf_alloc(dims, inds, vals, o)
     for m in range(3):
         out = S.mttkrp(m, R, csf.ptr, mats, o)
         assert rel_fro(out, gold[m]) < TOL, (R, m)
@@ -84,11 +69,13 @@ def test_ranks(S, refmod, R):
 @pytest.mark.parametrize("name", ["t3_mid", "t4", "t5"])
 @pytest.mark.parametrize("tilelevel", [0, 1, 2])
 def test_dropin_on_densetiled_reference_csf(S, refmod, name, tilelevel):
-    """Reference CSFs built with SPLATT_DENSETILE (tests/mttkrp_test.c:201-259)."""
+    """Reference CSFs built with SPLATT_DENSETILE (tests/mttkrp_test.c:201-259); only the
+    reference's csf_alloc builds them, so this runs where oracle/_ref is built."""
     dims, inds, vals = _tensor(name)
     R = 8
     mats = factor_mats(dims, R)
-    tt, gold = _gold(refmod, dims, inds, vals, mats)
+    tt = refmod.RefTensor.from_coo(dims, inds, vals)
+    gold = mttkrp_gold(dims, inds, vals, mats)
     for alloc in (0, 1, 2):
         o = refmod.default_opts()
         o[0] = 3
@@ -104,62 +91,45 @@ def test_dropin_on_densetiled_reference_csf(S, refmod, name, tilelevel):
 
 @pytest.mark.parametrize("name", ["t2_matrix", "t3_small", "t3_mid", "t4", "t5", "t8"])
 @pytest.mark.parametrize("alloc", [0, 1, 2])
-def test_csf_alloc_matches_reference(S, refmod, name, alloc):
+def test_csf_alloc_matches_reference(S, name, alloc):
     """splatt_b200_csf_alloc builds bit-identical CSF arrays to the reference's csf_alloc
-    (structure tests of tests/csf_test.c:31-61)."""
+    (structure tests of tests/csf_test.c:31-61): sizes, orders and a digest of every array
+    against the ones recorded from the reference."""
     dims, inds, vals = _tensor(name)
-    o = refmod.default_opts()
+    o = S.default_opts()
     o[0] = 1
     o[6] = alloc
-    tt = refmod.RefTensor.from_coo(dims, inds, vals)
-    rc = refmod.RefCsf(tt, o)
+    want = recorded.csf_digests(name, alloc)
     mine = S.csf_alloc(dims, inds, vals, o)
-    assert mine.count == rc.count
-    for c in range(rc.count):
-        a, b = mine.arrays(c), rc.arrays(c)
-        assert a["dim_perm"] == b["dim_perm"] and a["dim_iperm"] == b["dim_iperm"]
-        assert a["nfibs"] == b["nfibs"] and a["nnz"] == b["nnz"] and a["dims"] == b["dims"]
-        for l in range(len(dims)):
-            if b["fids"][l] is None:
-                assert a["fids"][l] is None
-            else:
-                assert np.array_equal(a["fids"][l], b["fids"][l]), (c, l)
-        for l in range(len(dims) - 1):
-            assert np.array_equal(a["fptr"][l], b["fptr"][l]), (c, l)
-        assert np.array_equal(a["vals"], b["vals"])
+    assert mine.count == len(want)
+    for c in range(mine.count):
+        assert recorded.csf_digest(mine.arrays(c)) == want[c], c
 
 
-def test_csf_alloc_gaps_keep_root_ids(S, refmod):
+def test_csf_alloc_gaps_keep_root_ids(S):
     """Empty root slices => fids[0] is materialised (src/csf.c:303-309)."""
     dims, inds, vals = random_coo((500, 40, 30), 300, seed=5)
-    o = refmod.default_opts()
+    o = S.default_opts()
     o[6] = 0
-    tt = refmod.RefTensor.from_coo(dims, inds, vals)
-    rc = refmod.RefCsf(tt, o)
     mine = S.csf_alloc(dims, inds, vals, o)
-    a, b = mine.arrays(0), rc.arrays(0)
-    assert a["dim_perm"] == b["dim_perm"]
-    for l in range(3):
-        assert (a["fids"][l] is None) == (b["fids"][l] is None)
-        if a["fids"][l] is not None:
-            assert np.array_equal(a["fids"][l], b["fids"][l])
+    a = mine.arrays(0)
+    assert recorded.csf_digest(a) == recorded.csf_digests("gaps", 0)[0]
     R = 4
     mats = factor_mats(dims, R)
-    gold = [tt.mttkrp_stream(mats, m) for m in range(3)]
+    gold = mttkrp_gold(dims, inds, vals, mats)
     for m in range(3):
         assert rel_fro(S.mttkrp(m, R, mine.ptr, mats, o), gold[m]) < TOL
-        assert rel_fro(S.mttkrp(m, R, rc.ptr, mats, o), gold[m]) < TOL
 
 
 @pytest.mark.parametrize("layout", [0, 1])
 @pytest.mark.parametrize("name", ["t2_matrix", "t3_mid", "t3_skew", "t4", "t5"])
-def test_engine_device_path(S, refmod, name, layout):
+def test_engine_device_path(S, name, layout):
     """Device-resident API: COO -> fiber streams -> MTTKRP on torch CUDA tensors."""
     import torch
     dims, inds, vals = _tensor(name)
     R = 16
     mats = factor_mats(dims, R)
-    _, gold = _gold(refmod, dims, inds, vals, mats)
+    gold = mttkrp_gold(dims, inds, vals, mats)
     T = S.Tensor.from_coo(dims, inds, vals, layout=layout, csf_alloc=1)
     dmats = [torch.from_numpy(m).cuda() for m in mats]
     for m in range(len(dims)):
@@ -175,14 +145,14 @@ def test_engine_device_path(S, refmod, name, layout):
 
 @pytest.mark.parametrize("name", ["t3_mid", "t3_long_fibers", "t3_skew", "t4", "t5"])
 @pytest.mark.parametrize("ktile", [1, 7, 64])
-def test_leaf_tiled_streams(S, refmod, name, ktile):
+def test_leaf_tiled_streams(S, name, ktile):
     """Leaf-tile re-ordered streams (the L1-reuse layout) give the same MTTKRP, for the
     root kernels and for the internal/leaf kernels, sharded or not."""
     import torch
     dims, inds, vals = _tensor(name)
     R = 16
     mats = factor_mats(dims, R)
-    _, gold = _gold(refmod, dims, inds, vals, mats)
+    gold = mttkrp_gold(dims, inds, vals, mats)
     dmats = [torch.from_numpy(m).cuda() for m in mats]
     for layout in (0, 1):
         for world in (1, 3):
@@ -203,7 +173,7 @@ def test_leaf_tiled_streams(S, refmod, name, ktile):
 @pytest.mark.parametrize("name", ["t3_small", "t3_mid", "t3_long_fibers", "t3_skew"])
 @pytest.mark.parametrize("rows", [1, 5, 37])
 @pytest.mark.parametrize("R", [2, 16, 32, 64])
-def test_cta_tiled_kernel(S, refmod, name, rows, R, monkeypatch):
+def test_cta_tiled_kernel(S, name, rows, R, monkeypatch):
     """The shared-memory leaf-tile kernel (mttkrp_tiled.cu), forced on small tensors with
     tiny tiles, sharded or not, against the reference's gold."""
     import torch
@@ -211,7 +181,7 @@ def test_cta_tiled_kernel(S, refmod, name, rows, R, monkeypatch):
     monkeypatch.setenv("SPLATT_B200_TILE_ROWS", str(rows))
     dims, inds, vals = _tensor(name)
     mats = factor_mats(dims, R)
-    _, gold = _gold(refmod, dims, inds, vals, mats)
+    gold = mttkrp_gold(dims, inds, vals, mats)
     dmats = [torch.from_numpy(m).cuda() for m in mats]
     for world in (1, 2):
         shards = [S.Tensor.from_coo(dims, inds, vals, shard_rank=r, shard_count=world,
@@ -229,14 +199,14 @@ def test_cta_tiled_kernel(S, refmod, name, rows, R, monkeypatch):
             s.free()
 
 
-def test_sharded_partials_sum_to_whole(S, refmod):
+def test_sharded_partials_sum_to_whole(S):
     """shard_count > 1: per-shard partial outputs add up to the full MTTKRP
     (what the NCCL all-reduce does across ranks)."""
     import torch
     dims, inds, vals = _tensor("t3_skew")
     R = 32
     mats = factor_mats(dims, R)
-    _, gold = _gold(refmod, dims, inds, vals, mats)
+    gold = mttkrp_gold(dims, inds, vals, mats)
     dmats = [torch.from_numpy(m).cuda() for m in mats]
     for world in (2, 3, 8):
         for layout in (0, 1):
@@ -255,7 +225,7 @@ def test_sharded_partials_sum_to_whole(S, refmod):
 @pytest.mark.parametrize("host_solve", ["0", "1"])
 @pytest.mark.parametrize("spec", [((60, 50, 40), 6000, 6), ((30, 25, 20, 15), 5000, 5),
                                   ((200, 150, 100), 30000, 16)])
-def test_cpd_als_tracks_reference(S, refmod, host_solve, spec, monkeypatch):
+def test_cpd_als_tracks_reference(S, host_solve, spec, monkeypatch):
     """CPD-ALS: same seed, same iteration count => same fit, lambda and factors, with the
     dense ALS tail on the device (default) and on the host (north-star wording).
     (The reference has no CPD result test; parity here is against the compiled
@@ -264,14 +234,13 @@ def test_cpd_als_tracks_reference(S, refmod, host_solve, spec, monkeypatch):
     dims, inds, vals = random_coo(spec[0], spec[1], seed=3)
     dims, inds, vals = cover_all_slices(dims, inds, vals)
     R = spec[2]
-    o = refmod.default_opts()
+    o = S.default_opts()
     o[0] = 1
     o[3] = 8          # iterations
     o[1] = 0.0        # tolerance: run them all
     o[4] = 0          # quiet
-    tt = refmod.RefTensor.from_coo(dims, inds, vals)
-    csf = refmod.RefCsf(tt, o)
-    fit_ref, lam_ref, fac_ref = csf.cpd_als(R, seed=7)
+    csf = S.csf_alloc(dims, inds, vals, o)
+    fit_ref, lam_ref, fac_ref = restate.cpd_als(dims, inds, vals, R, int(o[3]), float(o[1]), 7)
     fit, lam, fac = S.cpd_als(csf.ptr, R, o, seed=7)
     assert abs(fit - fit_ref) < 1e-8
     assert np.allclose(lam, lam_ref, rtol=1e-6, atol=1e-9)
@@ -279,33 +248,32 @@ def test_cpd_als_tracks_reference(S, refmod, host_solve, spec, monkeypatch):
         assert np.allclose(a, b, rtol=1e-5, atol=1e-8)
 
 
-def test_cpd_als_rank_deficient_falls_back(S, refmod):
+def test_cpd_als_rank_deficient_falls_back(S):
     """Duplicate factor columns cannot arise from random init, so force a singular normal
     matrix with rank > number of distinct rows: both the reference (GELSS) and we
     (pseudo-inverse) must return a finite fit and agree."""
     dims, inds, vals = random_coo((3, 40, 30), 600, seed=9)
     dims, inds, vals = cover_all_slices(dims, inds, vals)
-    o = refmod.default_opts()
+    o = S.default_opts()
     o[0], o[3], o[1], o[4] = 1, 3, 0.0, 0
-    tt = refmod.RefTensor.from_coo(dims, inds, vals)
-    csf = refmod.RefCsf(tt, o)
-    fit_ref, _, _ = csf.cpd_als(5, seed=2)      # rank 5 > dims[0] = 3: Gram of mode 0 singular
+    csf = S.csf_alloc(dims, inds, vals, o)
+    fit_ref, _, _ = restate.cpd_als(dims, inds, vals, 5, int(o[3]), float(o[1]), 2)      # rank 5 > dims[0] = 3: Gram of mode 0 singular
     fit, lam, fac = S.cpd_als(csf.ptr, 5, o, seed=2)
     assert np.isfinite(fit) and np.all(np.isfinite(lam))
     assert abs(fit - fit_ref) < 1e-6
 
 
 @pytest.mark.parametrize("R", [8, 17, 32, 70])
-def test_pinned_dropin_path(S, refmod, monkeypatch, R):
+def test_pinned_dropin_path(S, monkeypatch, R):
     """SPLATT_B200_PIN=1: caller buffers are page-locked on first sight; with page-locked
     buffers and >= 16 columns the call runs as a two-block column pipeline (PCIe copies of one
     block overlap the kernel of the other).  Same results; buffers released with the workspace."""
     monkeypatch.setenv("SPLATT_B200_PIN", "1")
     dims, inds, vals = _tensor("t3_mid")
     mats = factor_mats(dims, R)
-    tt, gold = _gold(refmod, dims, inds, vals, mats)
-    o = refmod.default_opts()
-    csf = refmod.RefCsf(tt, o)
+    gold = mttkrp_gold(dims, inds, vals, mats)
+    o = S.default_opts()
+    csf = S.csf_alloc(dims, inds, vals, o)
     for rep in range(2):                      # a second workspace re-registers the same buffers
         ws = S.MttkrpWorkspace(csf.ptr, R, o)
         outs = [np.empty((d, R)) for d in dims]
@@ -316,7 +284,7 @@ def test_pinned_dropin_path(S, refmod, monkeypatch, R):
         ws.free()
 
 
-def test_pinned_shared_maxdim_output(S, refmod, monkeypatch):
+def test_pinned_shared_maxdim_output(S, monkeypatch):
     """SPLATT_B200_PIN=1 with ONE output buffer of maxdim x R reused for every mode, smallest
     mode first -- what the reference's CPD driver does (src/cpd.c:322-327): the registration
     must grow with the extent actually used."""
@@ -324,9 +292,9 @@ def test_pinned_shared_maxdim_output(S, refmod, monkeypatch):
     dims, inds, vals = random_coo((40, 900, 300), 30000, seed=5)
     R = 16
     mats = factor_mats(dims, R)
-    tt, gold = _gold(refmod, dims, inds, vals, mats)
-    o = refmod.default_opts()
-    csf = refmod.RefCsf(tt, o)
+    gold = mttkrp_gold(dims, inds, vals, mats)
+    o = S.default_opts()
+    csf = S.csf_alloc(dims, inds, vals, o)
     ws = S.MttkrpWorkspace(csf.ptr, R, o)
     shared = np.empty((max(dims), R))
     for _ in range(2):
@@ -339,15 +307,15 @@ def test_pinned_shared_maxdim_output(S, refmod, monkeypatch):
 
 @pytest.mark.parametrize("stage", ["0", "1"])
 @pytest.mark.parametrize("R", [5, 32])
-def test_pageable_paths(S, refmod, monkeypatch, stage, R):
+def test_pageable_paths(S, monkeypatch, stage, R):
     """Pageable caller buffers: staged through the workspace's page-locked bounce buffers
     (default) or handed to cudaMemcpy directly (SPLATT_B200_STAGE=0)."""
     monkeypatch.setenv("SPLATT_B200_STAGE", stage)
     dims, inds, vals = _tensor("t3_skew")
     mats = factor_mats(dims, R)
-    tt, gold = _gold(refmod, dims, inds, vals, mats)
-    o = refmod.default_opts()
-    csf = refmod.RefCsf(tt, o)
+    gold = mttkrp_gold(dims, inds, vals, mats)
+    o = S.default_opts()
+    csf = S.csf_alloc(dims, inds, vals, o)
     ws = S.MttkrpWorkspace(csf.ptr, R, o)
     for _ in range(2):
         for m in range(3):
@@ -357,7 +325,7 @@ def test_pageable_paths(S, refmod, monkeypatch, stage, R):
     ws.free()
 
 
-def test_bare_mttkrp_reuses_device_mirror(S, refmod, monkeypatch):
+def test_bare_mttkrp_reuses_device_mirror(S, monkeypatch):
     """splatt_mttkrp (no workspace handle; matlab/splatt_mttkrp.c:68) builds the device
     mirror once per tensor: later calls find it in the cache (no stream build), a different
     tensor gets its own, and a tensor whose content changed in place is rebuilt."""
@@ -366,9 +334,9 @@ def test_bare_mttkrp_reuses_device_mirror(S, refmod, monkeypatch):
     dims, inds, vals = _tensor("t3_mid")
     R = 8
     mats = factor_mats(dims, R)
-    tt, gold = _gold(refmod, dims, inds, vals, mats)
-    o = refmod.default_opts()
-    csf = refmod.RefCsf(tt, o)
+    gold = mttkrp_gold(dims, inds, vals, mats)
+    o = S.default_opts()
+    csf = S.csf_alloc(dims, inds, vals, o)
     b0 = S.build_count()
     for rep in range(3):
         for m in range(3):
@@ -380,8 +348,8 @@ def test_bare_mttkrp_reuses_device_mirror(S, refmod, monkeypatch):
     # another tensor: its own mirror; the first one is still cached
     d2, i2, v2 = _tensor("t4")
     m2 = factor_mats(d2, R)
-    tt2, gold2 = _gold(refmod, d2, i2, v2, m2)
-    csf2 = refmod.RefCsf(tt2, o)
+    gold2 = mttkrp_gold(d2, i2, v2, m2)
+    csf2 = S.csf_alloc(d2, i2, v2, o)
     assert rel_fro(S.mttkrp(0, R, csf2.ptr, m2, o), gold2[0]) < TOL
     b2 = S.build_count()
     assert b2 - b1 == 4
@@ -408,17 +376,16 @@ def test_bare_mttkrp_reuses_device_mirror(S, refmod, monkeypatch):
 
 @pytest.mark.parametrize("R", [20, 32, 48, 64])
 @pytest.mark.parametrize("generic", ["0", "1"])
-def test_cpd_als_tail_kernels(S, refmod, monkeypatch, R, generic):
+def test_cpd_als_tail_kernels(S, monkeypatch, R, generic):
     """The register-tiled solve / SYRK kernels of the device tail (rank padded to 32 / 64) and
     the generic ones (SPLATT_B200_TAIL_GENERIC=1) against the compiled reference."""
     monkeypatch.setenv("SPLATT_B200_TAIL_GENERIC", generic)
     dims, inds, vals = random_coo((260, 150, 100), 40000, seed=17)
     dims, inds, vals = cover_all_slices(dims, inds, vals)
-    o = refmod.default_opts()
+    o = S.default_opts()
     o[0], o[3], o[1], o[4] = 4, 5, 0.0, 0
-    tt = refmod.RefTensor.from_coo(dims, inds, vals)
-    csf = refmod.RefCsf(tt, o)
-    fit_ref, lam_ref, fac_ref = csf.cpd_als(R, seed=9)
+    csf = S.csf_alloc(dims, inds, vals, o)
+    fit_ref, lam_ref, fac_ref = restate.cpd_als(dims, inds, vals, R, int(o[3]), float(o[1]), 9)
     fit, lam, fac = S.cpd_als(csf.ptr, R, o, seed=9)
     assert abs(fit - fit_ref) < 1e-8, (R, generic, fit, fit_ref)
     assert np.allclose(lam, lam_ref, rtol=1e-6, atol=1e-9)
@@ -426,32 +393,31 @@ def test_cpd_als_tail_kernels(S, refmod, monkeypatch, R, generic):
         assert np.allclose(a, b, rtol=1e-5, atol=1e-8)
 
 
-def test_cpd_als_rank_128_device_tail(S, refmod):
+def test_cpd_als_rank_128_device_tail(S):
     """Rank 128: the device tail's shared-memory needs (R*R + R*rows doubles for the row
     solve, R*R for the Cholesky) must be sized to the device, not assumed (round-1 advice):
     results still track the compiled reference."""
     dims, inds, vals = random_coo((300, 250, 200), 60000, seed=13)
     dims, inds, vals = cover_all_slices(dims, inds, vals)
     R = 128
-    o = refmod.default_opts()
+    o = S.default_opts()
     o[0], o[3], o[1], o[4] = 4, 3, 0.0, 0
-    tt = refmod.RefTensor.from_coo(dims, inds, vals)
-    csf = refmod.RefCsf(tt, o)
-    fit_ref, lam_ref, fac_ref = csf.cpd_als(R, seed=5)
+    csf = S.csf_alloc(dims, inds, vals, o)
+    fit_ref, lam_ref, fac_ref = restate.cpd_als(dims, inds, vals, R, int(o[3]), float(o[1]), 5)
     fit, lam, fac = S.cpd_als(csf.ptr, R, o, seed=5)
     assert np.isfinite(fit)
     assert abs(fit - fit_ref) < 1e-7, (fit, fit_ref)
     assert np.allclose(lam, lam_ref, rtol=1e-5, atol=1e-8)
 
 
-def test_alias_output_with_own_factor(S, refmod):
+def test_alias_output_with_own_factor(S):
     """matrices[mode] may alias matout (matlab/splatt_mttkrp.c:47-68)."""
     dims, inds, vals = _tensor("t3_mid")
     R = 8
     mats = factor_mats(dims, R)
-    tt, gold = _gold(refmod, dims, inds, vals, mats)
-    o = refmod.default_opts()
-    csf = refmod.RefCsf(tt, o)
+    gold = mttkrp_gold(dims, inds, vals, mats)
+    o = S.default_opts()
+    csf = S.csf_alloc(dims, inds, vals, o)
     ws = S.MttkrpWorkspace(csf.ptr, R, o)
     for m in range(3):
         mm = [x.copy() for x in mats]
@@ -461,11 +427,9 @@ def test_alias_output_with_own_factor(S, refmod):
 
 
 # ---------------------------------------------------------------------------------------
-# BASELINE.json sizes.  Gold: (1) the compiled reference's own mttkrp_csf on the same tensor
-# for the configurations it finishes in seconds with the host's threads (configs 2 and 3 at
-# full size -- tests/mttkrp_test.c:49-125 is the shape of that check; configs 4 and 5 at
-# their full 100 M / 200 M nonzeros are checked against the reference by bench.py at every
-# N, see `named_configs[*].parity_rel_fro`); (2) an independent fp64 formulation in plain
+# BASELINE.json sizes.  Gold: (1) the reference's gold (oracle/restate.c) on the same tensor
+# for the configurations it finishes in seconds on one host thread (configs 2 and 3 at full
+# size -- tests/mttkrp_test.c:49-125 is the shape of that check); (2) an independent fp64 formulation in plain
 # torch ops (gather rows, multiply, index_add); (3) size-independent properties (linearity in
 # the values, agreement of the root kernel with the internal/leaf kernels).
 # ---------------------------------------------------------------------------------------
@@ -506,9 +470,9 @@ FULL = {
 
 
 @pytest.mark.parametrize("name", ["config2_10K3_10M_R32", "config3_5K4_50M_R16"])
-def test_full_size_against_reference(S, refmod, name):
+def test_full_size_against_reference(S, name):
     """Full-size BASELINE configs 2 and 3: the CUDA path (device-resident engine AND the
-    drop-in C entry on the reference's own CSF) against the reference's mttkrp_csf."""
+    drop-in C entry on a CSF in the reference's layout) against the reference's gold."""
     import os
     import torch
     dims, nnz, R, zipf = FULL[name]
@@ -516,23 +480,22 @@ def test_full_size_against_reference(S, refmod, name):
     g = torch.Generator(device="cuda").manual_seed(5)
     mats = [torch.rand(d, R, device="cuda", dtype=torch.float64, generator=g) * 6 - 3 for d in dims]
     mats_h = [m.cpu().numpy() for m in mats]
-    o = refmod.default_opts()
+    ind_h = [i.cpu().numpy().astype(np.uint64) for i in ind]
+    vals_h = vals.cpu().numpy()
+    o = S.default_opts()
     o[0] = min(len(os.sched_getaffinity(0)), 32)
-    tt = refmod.RefTensor.from_coo(list(dims), [i.cpu().numpy().astype(np.uint64) for i in ind],
-                                   vals.cpu().numpy())
-    csf = refmod.RefCsf(tt, o)                                  # reference csf_alloc (TWOMODE)
+    csf = S.csf_alloc(list(dims), ind_h, vals_h, o)            # TWOMODE, the reference's layout
     T = S.Tensor.from_coo(dims, ind, vals)
     for m in range(len(dims)):
-        gold, _ = csf.mttkrp_csf(mats_h, m)
+        gold = restate.mttkrp_coo(list(dims), ind_h, vals_h, mats_h, m)
         out = torch.empty((dims[m], R), dtype=torch.float64, device="cuda")
         T.mttkrp(m, mats, out)
         assert rel_fro(out.cpu().numpy(), gold) < TOL, (name, m)
-        if m == 0:                                              # drop-in entry on the reference's CSF
+        if m == 0:                                              # drop-in entry on the host CSF
             assert rel_fro(S.mttkrp(m, R, csf.ptr, mats_h, o), gold) < TOL, (name, "dropin")
     S.cache_clear()
     T.free()
     csf.free()
-    tt.free()
 
 
 @pytest.mark.parametrize("name", list(FULL))
@@ -565,7 +528,7 @@ def test_full_size_against_torch_fp64(S, name):
         t.free()
 
 
-def test_degenerate_inputs(S, refmod):
+def test_degenerate_inputs(S):
     """Edge cases the reference's tests touch: a single nonzero, one long fiber, one
     dense slice, duplicate coordinates, nnz below one chunk and exactly on chunk edges."""
     import torch
@@ -585,8 +548,7 @@ def test_degenerate_inputs(S, refmod):
     for dims, inds, vals in cases:
         R = 6
         mats = factor_mats(dims, R)
-        tt = refmod.RefTensor.from_coo(dims, inds, vals)
-        gold = [tt.mttkrp_stream(mats, m) for m in range(len(dims))]
+        gold = mttkrp_gold(dims, inds, vals, mats)
         dm = [torch.from_numpy(x).cuda() for x in mats]
         for layout in (0, 1):
             T = S.Tensor.from_coo(dims, inds, vals, layout=layout, csf_alloc=0)
@@ -641,7 +603,7 @@ def _libc_rand_factors(dims, R, seed):
 
 
 @pytest.mark.parametrize("spec", [((60, 50, 40), 6000, 6), ((30, 25, 20, 15), 5000, 5)])
-def test_sharded_cpd_driver_matches_splatt_cpd_als(S, refmod, spec):
+def test_sharded_cpd_driver_matches_splatt_cpd_als(S, spec):
     """splatt_b200.parallel.cpd_als_sharded (MTTKRP -> exchange -> device tail through the
     splatt_b200_als_tail_* entry points; here world = 1) walks the same trajectory as
     splatt_cpd_als and as the compiled reference."""
@@ -650,11 +612,10 @@ def test_sharded_cpd_driver_matches_splatt_cpd_als(S, refmod, spec):
     dims, inds, vals = random_coo(spec[0], spec[1], seed=3)
     dims, inds, vals = cover_all_slices(dims, inds, vals)
     R, seed, its = spec[2], 7, 8
-    o = refmod.default_opts()
+    o = S.default_opts()
     o[0], o[3], o[1], o[4] = 1, its, 0.0, 0
-    tt = refmod.RefTensor.from_coo(dims, inds, vals)
-    csf = refmod.RefCsf(tt, o)
-    fit_ref, lam_ref, fac_ref = csf.cpd_als(R, seed=seed)
+    csf = S.csf_alloc(dims, inds, vals, o)
+    fit_ref, lam_ref, fac_ref = restate.cpd_als(dims, inds, vals, R, int(o[3]), float(o[1]), seed)
     init = [torch.from_numpy(a).cuda() for a in _libc_rand_factors(dims, R, seed)]
     T = S.Tensor.from_coo(dims, inds, vals)
     fit, lam, fac, times = parallel.cpd_als_sharded(T, R, init, float(np.sum(vals * vals)),

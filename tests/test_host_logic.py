@@ -6,9 +6,9 @@ import pytest
 
 from oracle import restate
 from splatt_b200 import _abi as A
+from tests import recorded
 
-DIMS = [[30, 10, 20], [10, 10, 10], [30, 10, 20, 10], [5, 4, 3, 2, 1], [7, 7, 3, 7, 3, 9],
-        [2425, 10816, 29567], [60114, 83826, 23034, 1132, 100], [4, 3, 5, 4, 3, 6, 2, 5]]
+DIMS = recorded.ORDER_DIMS
 
 
 def level_orders(lib, dims, alloc):
@@ -27,20 +27,23 @@ def test_level_orders_match_restatement(lib, dims, alloc):
 
 
 @pytest.mark.parametrize("dims", DIMS)
-def test_level_orders_match_compiled_reference(lib, refmod, dims):
-    """csf_find_mode_order (src/csf.c:694-726) for the orders csf_alloc uses (:770-814)."""
+def test_level_orders_match_compiled_reference(lib, dims):
+    """csf_find_mode_order (src/csf.c:694-726) for the orders csf_alloc uses (:770-814), as
+    recorded from the compiled reference."""
     n = len(dims)
-    small = refmod.mode_order(dims, refmod.CSF_SORTED_SMALLFIRST)
+    z, k = recorded.load(), DIMS.index(dims)
+    small = z[f"order{k}_small"].tolist()
+    minusone = z[f"order{k}_minusone"].tolist()        # CSF_SORTED_MINUSONE, one row per mode
     assert level_orders(lib, dims, 0)[0] == [small]
     two, mp = level_orders(lib, dims, 1)
     assert two[0] == small
-    assert two[1] == refmod.mode_order(dims, refmod.CSF_SORTED_MINUSONE, small[-1])
+    assert two[1] == minusone[small[-1]]
     assert mp == [1 if m == small[-1] else 0 for m in range(n)]
     allm, mp = level_orders(lib, dims, 2)
-    assert allm == [refmod.mode_order(dims, refmod.CSF_SORTED_MINUSONE, m) for m in range(n)]
+    assert allm == minusone
     assert mp == list(range(n))
     for which in range(4):
-        assert restate.mode_order(dims, which, n - 1) == refmod.mode_order(dims, which, n - 1)
+        assert restate.mode_order(dims, which, n - 1) == z[f"order{k}_last"][which].tolist()
 
 
 def test_bad_policy_is_rejected(lib):
@@ -61,7 +64,8 @@ def test_missing_library_fails_loudly(monkeypatch, tmp_path):
 def test_csf_to_coo_expands_reference_csfs(lib, refmod, spec, tile, alloc):
     """Host side of the device mirror: a reference CSF (untiled, or DENSETILE at any depth,
     built with 7 threads like tests/mttkrp_test.c -- up to 7^nmodes mostly empty tiles) expands
-    to exactly the tensor's nonzeros."""
+    to exactly the tensor's nonzeros.  Only the reference's csf_alloc builds tiled CSFs, so
+    this runs where oracle/_ref is built."""
     import time
     from tests.util import random_coo
     dims, inds, vals = random_coo(spec[0], spec[1], seed=4)
@@ -108,12 +112,13 @@ def test_multi_gpu_engine_rejects_bad_arguments(lib):
     """No GPU needed: argument checks come before any CUDA call."""
     out = C.c_void_p()
     devs = (C.c_int * 1)(0)
+    builds = lib.splatt_b200_build_count()          # earlier tests in the process may have built
     assert lib.splatt_b200_multi_create(None, 1, 8, devs, 1, 0, C.byref(out)) == A.SPLATT_ERROR_BADINPUT
     assert lib.splatt_b200_multi_mttkrp_host(None, 0, None, None) == A.SPLATT_ERROR_BADINPUT
     assert lib.splatt_b200_multi_info(None, None, None, None, None) == A.SPLATT_ERROR_BADINPUT
     lib.splatt_b200_multi_free(None)
-    lib.splatt_b200_cache_clear()                       # empty cache: a no-op
-    assert lib.splatt_b200_build_count() == 0
+    lib.splatt_b200_cache_clear()
+    assert lib.splatt_b200_build_count() == builds
 
 
 def test_every_environment_switch_is_documented():

@@ -5,36 +5,25 @@ On a 1-GPU box the engine is exercised with a device list that names the same GP
 (`SPLATT_B200_DEVICES=0,0`): shards, per-device streams, the event-ordered peer-memory
 reduce, the replicated ALS tail and the drop-in plumbing all run; only the NVLink multicast
 mapping and the in-kernel group barrier need two real GPUs -- those tests run when
-`torch.cuda.device_count() >= 2` (gpurun --gpus 2) and are skipped otherwise.
+`torch.cuda.device_count() >= 2` and are skipped otherwise.
 
-Gold: the compiled reference (oracle/_ref): mttkrp_stream for MTTKRP, its own splatt_cpd_als
-for CPD (reference shape of the distributed loop: src/mpi/mpi_cpd.c:627-804).
+Gold: the reference's gold mttkrp_stream for MTTKRP and its cpd_als for CPD (reference shape
+of the distributed loop: src/mpi/mpi_cpd.c:627-804), both as oracle/restate.c restates them
+(pinned to output recorded from the compiled reference by tests/test_oracle.py).  CSFs in the
+reference's layout come from splatt_b200_csf_alloc.  "t3_tiny" has fewer chunks than devices:
+empty shards.
 """
-import zlib
-
 import numpy as np
 import pytest
 
-from tests.util import cover_all_slices, factor_mats, random_coo, rel_fro
+from oracle import restate
+from tests.util import cover_all_slices, factor_mats, mttkrp_gold, parity_tensor, random_coo, rel_fro
 
 pytestmark = pytest.mark.gpu
 
 TOL = 1e-11
 
-TENSORS = {
-    "t3_mid": ((300, 200, 400), 20000),
-    "t3_skew": ((2000, 1500, 60), 40000),
-    "t4": ((40, 30, 50, 20), 15000),
-    "t5": ((12, 15, 10, 20, 9), 8000),
-    "t2_matrix": ((300, 500), 9000),
-    "t3_tiny": ((5, 4, 3), 20),          # fewer chunks than devices: empty shards
-}
-
-
-def _tensor(name):
-    dims, nnz = TENSORS[name]
-    skew = [1.0, 1.0, 0] if name == "t3_skew" else None
-    return random_coo(dims, nnz, seed=zlib.crc32(name.encode()) % 1000, skew=skew)
+_tensor = parity_tensor
 
 
 @pytest.fixture(scope="module")
@@ -48,14 +37,9 @@ def _ngpus():
     return torch.cuda.device_count()
 
 
-def _gold(refmod, dims, inds, vals, mats):
-    tt = refmod.RefTensor.from_coo(dims, inds, vals)
-    return tt, [tt.mttkrp_stream(mats, m) for m in range(len(dims))]
-
-
 @pytest.mark.parametrize("name", ["t3_mid", "t3_skew", "t4", "t5", "t2_matrix", "t3_tiny"])
 @pytest.mark.parametrize("world", [2, 3, 8])
-def test_sliced_shards_equal_rank_built_shards(S, refmod, name, world):
+def test_sliced_shards_equal_rank_built_shards(S, name, world):
     """splatt_b200_tensor_shard (slice a whole tensor, re-base node numbers) gives what a
     rank-local build with shard_rank/shard_count gives: same nnz, same node counts, same
     partial MTTKRP -- and the partials sum to the whole."""
@@ -63,7 +47,7 @@ def test_sliced_shards_equal_rank_built_shards(S, refmod, name, world):
     dims, inds, vals = _tensor(name)
     R = 16
     mats = factor_mats(dims, R)
-    _, gold = _gold(refmod, dims, inds, vals, mats)
+    gold = mttkrp_gold(dims, inds, vals, mats)
     dmats = [torch.from_numpy(m).cuda() for m in mats]
     whole = S.Tensor.from_coo(dims, inds, vals)
     acc = [torch.zeros((dims[m], R), dtype=torch.float64, device="cuda") for m in range(len(dims))]
@@ -103,16 +87,16 @@ def _devlists():
 
 @pytest.mark.parametrize("name", ["t3_mid", "t3_skew", "t4", "t2_matrix", "t3_tiny"])
 @pytest.mark.parametrize("R", [3, 16, 32, 70])
-def test_multi_mttkrp_host_matches_reference(S, refmod, name, R):
+def test_multi_mttkrp_host_matches_reference(S, name, R):
     """splatt_b200_multi_mttkrp_host on every available device list (duplicated single GPU;
     2/4/8 real GPUs with the fused multicast exchange) vs the reference's gold; repeated
     calls and a changing mode order exercise buffer re-use."""
     dims, inds, vals = _tensor(name)
     mats = factor_mats(dims, R)
-    tt, gold = _gold(refmod, dims, inds, vals, mats)
-    o = refmod.default_opts()
+    gold = mttkrp_gold(dims, inds, vals, mats)
+    o = S.default_opts()
     o[0] = 1
-    csf = refmod.RefCsf(tt, o)
+    csf = S.csf_alloc(dims, inds, vals, o)
     for devs in _devlists():
         mg = S.MultiGpu(csf.ptr, int(o[6]), R, devs)
         assert mg.ndevices == len(devs)
@@ -126,16 +110,16 @@ def test_multi_mttkrp_host_matches_reference(S, refmod, name, R):
 
 
 @pytest.mark.parametrize("devs", ["0,0", "0,0,0,0"])
-def test_dropin_symbols_honour_device_list(S, refmod, devs, monkeypatch):
+def test_dropin_symbols_honour_device_list(S, devs, monkeypatch):
     """SPLATT_B200_DEVICES routes splatt_mttkrp_alloc_ws / splatt_mttkrp_csf / splatt_mttkrp
     through the multi engine (row e' of the scope table: multi-GPU behind the C API)."""
     monkeypatch.setenv("SPLATT_B200_DEVICES", devs)
     dims, inds, vals = _tensor("t3_mid")
     R = 16
     mats = factor_mats(dims, R)
-    tt, gold = _gold(refmod, dims, inds, vals, mats)
-    o = refmod.default_opts()
-    csf = refmod.RefCsf(tt, o)
+    gold = mttkrp_gold(dims, inds, vals, mats)
+    o = S.default_opts()
+    csf = S.csf_alloc(dims, inds, vals, o)
     ws = S.MttkrpWorkspace(csf.ptr, R, o)
     outs = [np.empty((d, R)) for d in dims]
     for _ in range(2):
@@ -148,16 +132,16 @@ def test_dropin_symbols_honour_device_list(S, refmod, devs, monkeypatch):
     csf.free()
 
 
-def test_dropin_ngpus_env_on_real_gpus(S, refmod, monkeypatch):
+def test_dropin_ngpus_env_on_real_gpus(S, monkeypatch):
     if _ngpus() < 2:
-        pytest.skip("needs >= 2 GPUs (gpurun --gpus 2)")
+        pytest.skip("needs >= 2 GPUs")
     monkeypatch.setenv("SPLATT_B200_NGPUS", str(min(_ngpus(), 8)))
     dims, inds, vals = _tensor("t3_skew")
     R = 32
     mats = factor_mats(dims, R)
-    tt, gold = _gold(refmod, dims, inds, vals, mats)
-    o = refmod.default_opts()
-    csf = refmod.RefCsf(tt, o)
+    gold = mttkrp_gold(dims, inds, vals, mats)
+    o = S.default_opts()
+    csf = S.csf_alloc(dims, inds, vals, o)
     ws = S.MttkrpWorkspace(csf.ptr, R, o)
     outs = [np.empty((d, R)) for d in dims]
     for _ in range(3):
@@ -170,17 +154,16 @@ def test_dropin_ngpus_env_on_real_gpus(S, refmod, monkeypatch):
 
 @pytest.mark.parametrize("spec", [((60, 50, 40), 6000, 6), ((30, 25, 20, 15), 5000, 5),
                                   ((200, 150, 100), 30000, 16)])
-def test_multi_cpd_als_tracks_reference(S, refmod, spec):
+def test_multi_cpd_als_tracks_reference(S, spec):
     """CPD-ALS over several devices: same seed and iteration count as the compiled reference
     => same fit / lambda / factors (the tolerances of the single-GPU CPD test)."""
     dims, inds, vals = random_coo(spec[0], spec[1], seed=3)
     dims, inds, vals = cover_all_slices(dims, inds, vals)
     R = spec[2]
-    o = refmod.default_opts()
+    o = S.default_opts()
     o[0], o[3], o[1], o[4] = 1, 8, 0.0, 0
-    tt = refmod.RefTensor.from_coo(dims, inds, vals)
-    csf = refmod.RefCsf(tt, o)
-    fit_ref, lam_ref, fac_ref = csf.cpd_als(R, seed=7)
+    csf = S.csf_alloc(dims, inds, vals, o)
+    fit_ref, lam_ref, fac_ref = restate.cpd_als(dims, inds, vals, R, int(o[3]), float(o[1]), 7)
     for devs in _devlists():
         mg = S.MultiGpu(csf.ptr, int(o[6]), R, devs)
         fit, lam, fac = mg.cpd_als(o, seed=7)
@@ -192,14 +175,13 @@ def test_multi_cpd_als_tracks_reference(S, refmod, spec):
     csf.free()
 
 
-def test_splatt_cpd_als_honours_device_list(S, refmod, monkeypatch):
+def test_splatt_cpd_als_honours_device_list(S, monkeypatch):
     dims, inds, vals = random_coo((60, 50, 40), 6000, seed=3)
     dims, inds, vals = cover_all_slices(dims, inds, vals)
-    o = refmod.default_opts()
+    o = S.default_opts()
     o[0], o[3], o[1], o[4] = 1, 6, 0.0, 0
-    tt = refmod.RefTensor.from_coo(dims, inds, vals)
-    csf = refmod.RefCsf(tt, o)
-    fit_ref, _, _ = csf.cpd_als(6, seed=11)
+    csf = S.csf_alloc(dims, inds, vals, o)
+    fit_ref, _, _ = restate.cpd_als(dims, inds, vals, 6, int(o[3]), float(o[1]), 11)
     n = _ngpus()
     monkeypatch.setenv("SPLATT_B200_DEVICES", "0,1" if n >= 2 else "0,0")
     fit, lam, fac = S.cpd_als(csf.ptr, 6, o, seed=11)
@@ -207,18 +189,17 @@ def test_splatt_cpd_als_honours_device_list(S, refmod, monkeypatch):
     csf.free()
 
 
-def test_multi_cpd_factors_stay_single_valued(S, refmod):
+def test_multi_cpd_factors_stay_single_valued(S):
     """An ill-conditioned problem (rank 32 on a 300^3 random tensor): with a tail replicated
     on every device the factor replicas drift apart within ~10 iterations and the fit blows up
-    (measured on 2 GPUs).  The engine runs the tail once and hands the factor to the other
+    (seen on 2 GPUs).  The engine runs the tail once and hands the factor to the other
     devices, so many iterations later it still tracks the single-GPU run."""
     dims, inds, vals = random_coo((300, 300, 300), 200000, seed=21)
     dims, inds, vals = cover_all_slices(dims, inds, vals)
     R = 32
-    o = refmod.default_opts()
+    o = S.default_opts()
     o[0], o[3], o[1], o[4] = 1, 16, 0.0, 0
-    tt = refmod.RefTensor.from_coo(dims, inds, vals)
-    csf = refmod.RefCsf(tt, o)
+    csf = S.csf_alloc(dims, inds, vals, o)
     fit1, _, _ = S.cpd_als(csf.ptr, R, o, seed=3)
     assert 0.0 < fit1 < 1.0
     for devs in _devlists():
@@ -229,16 +210,15 @@ def test_multi_cpd_factors_stay_single_valued(S, refmod):
     csf.free()
 
 
-def test_real_gpus_use_the_multicast_exchange(S, refmod):
+def test_real_gpus_use_the_multicast_exchange(S):
     """On an NVSwitch box the engine must come up with the fused multicast exchange (the
     peer-reduce path is only the fallback); SPLATT_B200_MULTICAST=0 forces the fallback."""
     import os
     if _ngpus() < 2:
-        pytest.skip("needs >= 2 GPUs (gpurun --gpus 2)")
+        pytest.skip("needs >= 2 GPUs")
     dims, inds, vals = _tensor("t3_mid")
-    tt = refmod.RefTensor.from_coo(dims, inds, vals)
-    o = refmod.default_opts()
-    csf = refmod.RefCsf(tt, o)
+    o = S.default_opts()
+    csf = S.csf_alloc(dims, inds, vals, o)
     mg = S.MultiGpu(csf.ptr, int(o[6]), 8, [0, 1])
     assert mg.multicast or os.environ.get("SPLATT_B200_MULTICAST") == "0"
     mg.free()
@@ -247,7 +227,7 @@ def test_real_gpus_use_the_multicast_exchange(S, refmod):
         mg = S.MultiGpu(csf.ptr, int(o[6]), 8, [0, 1])
         assert not mg.multicast
         mats = factor_mats(dims, 8)
-        gold = tt.mttkrp_stream(mats, 1)
+        gold = restate.mttkrp_coo(dims, inds, vals, mats, 1)
         assert rel_fro(mg.mttkrp_host(1, mats), gold) < TOL
         mg.free()
     finally:

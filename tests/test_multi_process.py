@@ -4,7 +4,7 @@ CPD-ALS with either exchange -- scripts/test_fused.py under torchrun, which asse
   * fused == NCCL result to 1e-12 over 20 sweeps x 3 modes (the in-kernel barrier must order
     the remote reductions every time),
   * identical CPD fits with both exchanges.
-Needs >= 2 GPUs (gpurun --gpus 2); skipped on the 1-GPU box."""
+Needs >= 2 GPUs; skipped on a machine with one."""
 import re
 import subprocess
 import sys
@@ -20,7 +20,7 @@ def test_fused_exchange_and_sharded_cpd_under_torchrun():
     import torch
     n = torch.cuda.device_count()
     if n < 2:
-        pytest.skip("needs >= 2 GPUs (gpurun --gpus 2)")
+        pytest.skip("needs >= 2 GPUs")
     r = subprocess.run([sys.executable, "-m", "torch.distributed.run", "--nnodes=1",
                         "--nproc-per-node", "2", "--master-addr", "127.0.0.1", "--master-port",
                         "29531", str(ROOT / "scripts" / "test_fused.py")],

@@ -4,8 +4,9 @@
     the reference's own gold (mttkrp_stream) on the reference's own fixtures
     (tests/golden/make_golden.py).  Tolerance = the reference's own test
     tolerance, abs 1e-10 (tests/mttkrp_test.c:25-30), plus 1e-12 relative.
-(2) oracle/restate.c against the compiled reference (oracle/_ref) on seeded
-    random tensors: CSF arrays bit-exact, MTTKRP (COO and CSF walk) 1e-12.
+(2) oracle/restate.c against output recorded from the compiled reference
+    (tests/recorded.py) on seeded random tensors: CSF arrays bit-exact, MTTKRP (COO and
+    CSF walk) 1e-12, CPD-ALS on every problem the GPU tests solve.
 """
 from pathlib import Path
 
@@ -13,7 +14,8 @@ import numpy as np
 import pytest
 
 from oracle import restate
-from tests.util import cover_all_slices, factor_mats, random_coo, rel_fro
+from tests import recorded
+from tests.util import factor_mats, random_coo, rel_fro
 
 GOLD = Path(__file__).parent / "golden"
 NAMES = ["small", "med", "small4", "med4", "med5", "small4_zeroidx"]
@@ -70,63 +72,47 @@ def test_zero_index_fixture_equals_one_index_fixture():
         assert np.array_equal(a, b)
 
 
-SPECS = [((30, 50), 700), ((13, 7, 11), 150), ((40, 30, 50, 20), 5000), ((12, 15, 10, 20, 9), 3000),
-         ((5, 6, 4, 7, 3, 5), 1500)]
+SPECS = recorded.ORACLE_SPECS
 
 
 @pytest.mark.parametrize("spec", SPECS)
 @pytest.mark.parametrize("alloc", [0, 1, 2])
-def test_restatement_vs_compiled_reference(refmod, spec, alloc):
+def test_restatement_vs_compiled_reference(spec, alloc):
+    k = SPECS.index(spec)
     dims, inds, vals = random_coo(spec[0], spec[1], seed=11)
     mats = factor_mats(dims, 5)
-    tt = refmod.RefTensor.from_coo(dims, inds, vals)
-    gold = [tt.mttkrp_stream(mats, m) for m in range(len(dims))]
+    z = recorded.load()
+    gold = [z[f"spec{k}_m{m}"] for m in range(len(dims))]
     perms, mode_map = restate.csf_policy(dims, alloc)
-    o = refmod.default_opts()
-    o[0] = 2
-    o[6] = alloc
-    rc = refmod.RefCsf(tt, o)
-    assert rc.count == len(perms)
+    want = recorded.csf_digests(f"spec{k}", alloc)
+    assert len(want) == len(perms)
     for c, perm in enumerate(perms):
         oc = restate.OracleCsf(dims, inds, vals, perm)
-        a, b = oc.arrays(), rc.arrays(c)
-        assert a["dim_perm"] == b["dim_perm"] and a["nfibs"] == b["nfibs"]
-        for l in range(len(dims)):
-            assert (a["fids"][l] is None) == (b["fids"][l] is None)
-            if a["fids"][l] is not None:
-                assert np.array_equal(a["fids"][l], b["fids"][l])
-        for l in range(len(dims) - 1):
-            assert np.array_equal(a["fptr"][l], b["fptr"][l])
-        assert np.array_equal(a["vals"], b["vals"])
+        got = recorded.csf_digest(oc.arrays())
+        assert got == {key: want[c][key] for key in got}, c
         for m in range(len(dims)):
             assert rel_fro(oc.mttkrp(mats, m), gold[m]) < 1e-12
     for m in range(len(dims)):
         assert rel_fro(restate.mttkrp_coo(dims, inds, vals, mats, m), gold[m]) < 1e-13
-        if len(dims) > 2:
-            # reference production path == reference gold.  (For matrices the reference's CSF
-            # leaf-mode kernel does not reproduce its own gold -- src/mttkrp.c:860-943 assumes
-            # nmodes >= 3 -- so 2-mode parity is anchored on the COO gold only.)
-            out, _ = rc.mttkrp_csf(mats, m)
-            assert rel_fro(out, gold[m]) < 1e-12
 
 
-def test_restatement_cpd_vs_compiled_reference(refmod):
-    dims, inds, vals = random_coo((60, 50, 40), 6000, seed=3)
-    dims, inds, vals = cover_all_slices(dims, inds, vals)
-    o = refmod.default_opts()
-    o[0], o[3], o[1], o[4] = 1, 8, 0.0, 0
-    tt = refmod.RefTensor.from_coo(dims, inds, vals)
-    rc = refmod.RefCsf(tt, o)
-    f1, l1, F1 = rc.cpd_als(6, 7)
-    f2, l2, F2 = restate.cpd_als(dims, inds, vals, 6, 8, 0.0, 7)
-    assert abs(f1 - f2) < 1e-12
-    assert np.allclose(l1, l2, rtol=1e-10)
-    for a, b in zip(F1, F2):
-        assert np.allclose(a, b, rtol=1e-9, atol=1e-12)
+def test_restatement_cpd_vs_compiled_reference():
+    dims, inds, vals = recorded.cpd_tensor("s3")
+    recorded.check_cpd("s3", *restate.cpd_als(dims, inds, vals, 6, 8, 0.0, 7))
+
+
+@pytest.mark.parametrize("key", list(recorded.CPD_CASES))
+def test_restatement_cpd_matches_recorded_reference(key):
+    """Every CPD-ALS problem the GPU tests check against the restatement: the restatement
+    reproduces the reference's fit, lambda and factors on it."""
+    _, _, R, _, its, seed = recorded.CPD_CASES[key]
+    dims, inds, vals = recorded.cpd_tensor(key)
+    recorded.check_cpd(key, *restate.cpd_als(dims, inds, vals, R, its, 0.0, seed))
 
 
 def test_compiled_reference_matches_golden(refmod):
-    """The compiled reference reproduces the committed vectors (guards the build flags)."""
+    """The compiled reference reproduces the committed vectors (guards the build flags of
+    oracle/build_ref.sh; runs where oracle/_ref is built)."""
     z, dims, inds, vals = load_golden("med")
     tt = refmod.RefTensor.from_coo(dims, inds, vals)
     mats = factor_mats(dims, 3, seed=3)

@@ -30,8 +30,6 @@ def _write_fixtures():
     FIX.mkdir(exist_ok=True)
     for name in ("small", "med", "small4", "med4", "med5"):
         out = FIX / f"{name}.tns"
-        if out.exists():
-            continue
         z = np.load(GOLD / f"{name}.npz")
         ind, vals = z["ind"], z["vals"]
         with open(out, "w") as f:

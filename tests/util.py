@@ -57,3 +57,32 @@ def factor_mats(dims, R, seed=0):
 def rel_fro(a, b):
     den = np.linalg.norm(b)
     return float(np.linalg.norm(a - b) / (den if den > 0 else 1.0))
+
+
+# Seeded tensors of the GPU parity tests (dims, nnz); "t3_skew" has Zipf(1) modes 0 and 1.
+PARITY_TENSORS = {
+    "t2_matrix": ((300, 500), 9000),
+    "t3_small": ((13, 7, 11), 150),
+    "t3_tiny": ((5, 4, 3), 20),
+    "t3_mid": ((300, 200, 400), 20000),
+    "t3_long_fibers": ((50, 40, 3000), 30000),
+    "t3_skew": ((2000, 1500, 60), 40000),
+    "t4": ((40, 30, 50, 20), 15000),
+    "t5": ((12, 15, 10, 20, 9), 8000),
+    "t6": ((6, 7, 5, 8, 9, 4), 4000),
+    "t8": ((4, 3, 5, 4, 3, 6, 2, 5), 3000),
+}
+
+
+def parity_tensor(name):
+    import zlib
+    dims, nnz = PARITY_TENSORS[name]
+    skew = [1.0, 1.0, 0] if name == "t3_skew" else None
+    return random_coo(dims, nnz, seed=zlib.crc32(name.encode()) % 1000, skew=skew)   # stable seed
+
+
+def mttkrp_gold(dims, inds, vals, mats):
+    """Every mode's MTTKRP from oracle/restate.c, the restatement of the reference's gold
+    mttkrp_stream that tests/test_oracle.py pins to output recorded from the reference."""
+    from oracle import restate
+    return [restate.mttkrp_coo(dims, inds, vals, mats, m) for m in range(len(dims))]
