@@ -245,10 +245,10 @@ typedef struct
                             nnz-balanced share of every stream             */
   int32_t verbosity;     /* SPLATT_VERBOSITY_*                             */
   int32_t ncolumns_hint; /* rank the tensor will be used with (0 = unknown);
-                            lets the builder size leaf tiles for L1          */
-  int32_t ktile;         /* leaf-tile re-ordering: 0 = automatic (on when
-                            every leaf row would be re-used >= 3x per SM),
-                            -1 = off, > 0 = this many rows per tile          */
+                            not needed by the leaf-tiling policy            */
+  int32_t ktile;         /* leaf-tile re-ordering: 0 = automatic (shared-
+                            memory tiles where splatt_b200_cta_tiling says
+                            so), -1 = off, > 0 = this many rows per tile    */
   int32_t reserved[9];
 } splatt_b200_build_opts;
 
@@ -305,6 +305,18 @@ void splatt_b200_csf_free(splatt_csf * csf, int csf_alloc);
  * Returns the number of CSFs, 0 on a bad policy. */
 int splatt_b200_level_orders(
     uint64_t const * dims, int nmodes, int csf_alloc, int * perms, int * mode_csf_map);
+
+/* Host logic, no GPU needed: whether the stream with level order perm (root .. leaf) is built
+ * CTA-tiled, i.e. multiplied at its root by the kernel that serves leaf-factor rows from
+ * shared memory.  Needs 3 modes, an unsharded build, a stream whose every mode runs the
+ * root kernel (root_only), leaf rows re-used >= 3x by one SM's nonzeros, enough nonzeros per
+ * (root slice, leaf tile) piece, and an accumulator for a range's root rows that fits beside
+ * the tiles.  force = 1 skips the performance rules (testing).  Returns 1 and the tile and
+ * accumulator rows if so, 0 otherwise.  The build still falls back to an untiled stream when
+ * a range spans more root rows than *acc_rows. */
+int splatt_b200_cta_tiling(
+    int nmodes, uint64_t const * dims, int const * perm, uint64_t nnz_local, int shard_count,
+    int root_only, int num_sms, int force, uint32_t * tile_rows, uint32_t * acc_rows);
 
 /* Host logic, no GPU needed: the records [first, first+count) of a sorted stream
  * of `nnz` nonzeros that shard `rank` of `count_shards` keeps (equal numbers of

@@ -96,7 +96,7 @@ EXPORTS = [
     "splatt_b200_tensor_from_csf", "splatt_b200_tensor_from_coo", "splatt_b200_tensor_free",
     "splatt_b200_tensor_info", "splatt_b200_mode_info", "splatt_b200_csf_alloc",
     "splatt_b200_csf_free", "splatt_b200_mttkrp", "splatt_b200_launch_count",
-    "splatt_b200_version", "splatt_b200_level_orders", "splatt_b200_shard_range", "splatt_b200_mttkrp_multicast", "splatt_b200_gather_probe", "splatt_b200_gather_probe_ex", "splatt_b200_mttkrp_columns",
+    "splatt_b200_version", "splatt_b200_level_orders", "splatt_b200_cta_tiling", "splatt_b200_shard_range", "splatt_b200_mttkrp_multicast", "splatt_b200_gather_probe", "splatt_b200_gather_probe_ex", "splatt_b200_mttkrp_columns",
     "splatt_b200_als_tail_create", "splatt_b200_als_tail_free", "splatt_b200_als_tail_gram",
     "splatt_b200_als_tail_update", "splatt_b200_als_tail_fit", "splatt_b200_csf_to_coo",
     "splatt_b200_tensor_shard", "splatt_b200_mttkrp_multicast_sync",
@@ -230,6 +230,10 @@ def load() -> C.CDLL:
     lib.splatt_b200_level_orders.restype = C.c_int
     lib.splatt_b200_level_orders.argtypes = [idx_p, C.c_int, C.c_int, C.POINTER(C.c_int),
                                              C.POINTER(C.c_int)]
+    lib.splatt_b200_cta_tiling.restype = C.c_int
+    lib.splatt_b200_cta_tiling.argtypes = [C.c_int, idx_p, C.POINTER(C.c_int), C.c_uint64, C.c_int,
+                                           C.c_int, C.c_int, C.c_int, C.POINTER(C.c_uint32),
+                                           C.POINTER(C.c_uint32)]
     lib.splatt_b200_shard_range.restype = None
     lib.splatt_b200_shard_range.argtypes = [C.c_uint64, C.c_int, C.c_int, idx_p, idx_p]
     _lib = lib

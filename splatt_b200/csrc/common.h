@@ -38,6 +38,9 @@
 #define SPB200_CHUNK 64u             // records per descriptor chunk
 #define SPB200_IDX_BITS 29           // parent index bits in rec.aux
 #define SPB200_IDX_MASK 0x1fffffffu
+// CTA tiling pays only when a (root slice, leaf tile) piece holds this many nonzeros on
+// average: every piece ends a slice partial sum and splits fibers
+#define SPB200_MIN_NNZ_PER_PIECE 8.0
 
 struct __align__(16) SpRec {
   double   v;
@@ -64,7 +67,9 @@ struct FiberStream {
   // CTA-tiled variant (one range per CTA, leaf tile staged in shared memory):
   uint32_t * seg_off = nullptr;            // [kranges * ntiles + 1] first record of every segment
   uint32_t * rootid = nullptr;             // [nrec] root index of every record
+  uint32_t * rroot = nullptr;              // [2 * kranges] first / last root index of every range
   uint32_t ntiles = 0;
+  uint32_t acc_rows = 0;                   // rows of the kernel's shared accumulator
   uint64_t leaf_rows = 0;                  // rows of the leaf-mode factor
 };
 
@@ -72,7 +77,8 @@ struct FiberStream {
 struct StreamTiling {
   uint32_t tile_rows = 0;
   uint32_t nranges = 0;
-  bool     cta = false;      // build seg_off / rootid for the shared-memory tile kernel
+  bool     cta = false;      // build seg_off / rootid / rroot for the shared-memory tile kernel
+  uint32_t acc_rows = 0;     // cta: root rows the kernel can accumulate per range
 };
 
 enum { SPB200_KIND_ROOT = 0, SPB200_KIND_INTL = 1, SPB200_KIND_LEAF = 2 };
@@ -180,11 +186,13 @@ extern unsigned long long g_spb200_builds;     // fiber streams built (sort + sc
 inline void spb200_count_launches(unsigned n) { __atomic_fetch_add(&g_spb200_launches, n, __ATOMIC_RELAXED); }
 
 // mttkrp_tiled.cu -- 3-mode root kernel with the leaf factor staged tile by tile in smem
-bool spb200_tiled_applicable(const FiberStream & s, int kind, int ncolumns, int ldm);
-int spb200_launch_tiled_root3(const FiberStream & s, int ncolumns, int ldm, uint64_t leaf_rows,
+bool spb200_tiled_applicable(const FiberStream & s, int kind);
+// columns [col_begin, col_end) (even bounds) of the output
+int spb200_launch_tiled_root3(const FiberStream & s, int ldm, int col_begin, int col_end,
                               const double * leaf, const double * parent, double * d_out,
                               cudaStream_t stream);
-uint32_t spb200_tiled_rows_for(int ncolumns);   // rows of a leaf tile that fit the kernel's smem
+// rows of a leaf tile that fit the kernel's smem beside an accumulator of acc_rows rows
+uint32_t spb200_tiled_rows_for(uint32_t acc_rows);
 
 // cpd.cu -- row-partitioned ALS tail steps (multi-GPU engine).  Every device works on its own
 // row slice; partial column norms / Grams go to per-device slots of the multicast region and

@@ -373,6 +373,9 @@ splatt_mttkrp_ws * splatt_mttkrp_alloc_ws(splatt_csf const * const tensors,
   bo.layout = layout_from_env();
   bo.device = -1;
   bo.verbosity = (int)opts[SPLATT_OPTION_VERBOSITY];
+  // untiled streams: the copy/compute pipeline launches column blocks, and the tiled kernel
+  // re-walks every record per block (measured slower on config 2 with page-locked buffers)
+  bo.ktile = -1;
   if (splatt_b200_tensor_from_csf(tensors, csf_alloc, &bo, &w->T) != SPLATT_SUCCESS) {
     free_priv(w);
     return nullptr;

@@ -197,51 +197,53 @@ int build_tensor(int N, const uint64_t * dims, const DevCoo & dc,
   int num_sms = 132;
   cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, T->device);
   for (size_t i = 0; i < stream_perms.size(); ++i) {
-    // Leaf-tile re-ordering policy.  Worth it only when a leaf row is re-used several
-    // times by the nonzeros one SM processes (otherwise every row is fetched once
-    // anyway) and the leaf factor does not already fit in L1.
-    StreamTiling tiling;
-    // Two leaf-tiling layouts (both keep the stream valid for the generic kernels):
-    //  (a) CTA-tiled (opt-in, SPLATT_B200_TILED=1): one range per SM, leaf tiles staged in
-    //      shared memory by mttkrp_tiled.cu -- for 3-mode root streams when the rank is known
-    //      and every leaf row is re-used >= 3x by the nonzeros of one SM.  Measured slower
-    //      than the generic kernel on config 2 (DESIGN.md 4.3): the L1 data pipe, which
-    //      serves shared-memory reads too, is the wall;
+    // Leaf-tile re-ordering.  Two layouts, both valid for the generic kernels too:
+    //  (a) CTA-tiled: one range per SM, leaf tiles staged in shared memory by
+    //      mttkrp_tiled.cu; chosen by splatt_b200_cta_tiling (DESIGN.md 4.1);
     //  (b) L1-tiled (opt-in, ktile > 0): many small ranges, tiles kept hot in L1 only
     //      statistically -- measured not to pay off (DESIGN.md 4.3).
+    StreamTiling tiling;
+    uint64_t local = 0;
     {
-      const uint64_t leaf_dim = dims[stream_perms[i].perm[N - 1]];
       uint64_t c0, c1;
       spb200_shard_chunks(dc.nnz, T->shard_rank, T->shard_count, &c0, &c1);
-      const uint64_t local = std::min<uint64_t>(c1 * SPB200_CHUNK, dc.nnz) - c0 * SPB200_CHUNK;
+      local = std::min<uint64_t>(c1 * SPB200_CHUNK, dc.nnz) - c0 * SPB200_CHUNK;
+    }
+    if (bo.ktile > 0) {
+      tiling.tile_rows = (uint32_t)bo.ktile;
+      tiling.nranges = (uint32_t)num_sms * 48u;
+    } else if (bo.ktile == 0) {
+      bool root_only = true;            // every mode served by this stream runs the root kernel
+      for (int m = 0; m < N; ++m)
+        if (plan[m].stream == (int)i && plan[m].kind != SPB200_KIND_ROOT) root_only = false;
       const char * te = getenv("SPLATT_B200_TILED");
-      const bool tiled_ok = te && atoi(te) >= 1;     // opt-in: measured slower than the generic kernel
-      if (bo.ktile > 0) {
-        tiling.tile_rows = (uint32_t)bo.ktile;
-        tiling.nranges = (uint32_t)num_sms * 48u;
-      } else if (bo.ktile == 0 && tiled_ok && N == 3 && bo.ncolumns_hint > 0 &&
-                 bo.ncolumns_hint <= 64) {
-        uint32_t rows = spb200_tiled_rows_for(bo.ncolumns_hint);
+      const int force = (te && atoi(te) == 2) ? 1 : 0;             // testing: ignore the heuristics
+      uint32_t rows = 0, acc = 0;
+      if (splatt_b200_cta_tiling(N, dims, stream_perms[i].perm, local, T->shard_count,
+                                 root_only ? 1 : 0, num_sms, force, &rows, &acc)) {
         const char * re = getenv("SPLATT_B200_TILE_ROWS");          // testing / tuning
         if (re && atoi(re) > 0) rows = std::min<uint32_t>(rows, (uint32_t)atoi(re));
-        const bool force = te && atoi(te) == 2;                      // testing: ignore the heuristics
-        const double reuse = (double)local / num_sms / (double)std::max<uint64_t>(leaf_dim, 1);
-        if (force ? (rows >= 1 && local > 0)
-                  : (rows >= 16 && leaf_dim > rows && reuse >= 3.0 &&
-                     local >= (uint64_t)num_sms * 4096)) {
-          tiling.tile_rows = rows;
-          tiling.nranges = (uint32_t)num_sms;
-          tiling.cta = true;
-        }
+        tiling.tile_rows = rows;
+        tiling.nranges = (uint32_t)num_sms;
+        tiling.cta = true;
+        tiling.acc_rows = acc;
       }
-      if (tiling.tile_rows) {
-        const uint64_t ntiles = (leaf_dim + tiling.tile_rows - 1) / tiling.tile_rows;
-        if ((uint64_t)tiling.nranges * ntiles >= 0x7fffffffull) tiling = StreamTiling();
-      }
+    }
+    if (tiling.tile_rows) {
+      const uint64_t leaf_dim = dims[stream_perms[i].perm[N - 1]];
+      const uint64_t ntiles = (leaf_dim + tiling.tile_rows - 1) / tiling.tile_rows;
+      if ((uint64_t)tiling.nranges * ntiles >= 0x7fffffffull) tiling = StreamTiling();
     }
     int rc = spb200_build_stream(N, dims, dc.nnz, dc.ind, dc.vals, stream_perms[i].perm,
                                  stream_perms[i].presorted, T->shard_rank, T->shard_count,
                                  tiling, &T->streams[i]);
+    if (rc == SPLATT_SUCCESS && tiling.cta && T->streams[i].acc_rows > tiling.acc_rows) {
+      // a range touches more root rows than the shared accumulator holds: build it untiled
+      spb200_free_stream(&T->streams[i]);
+      rc = spb200_build_stream(N, dims, dc.nnz, dc.ind, dc.vals, stream_perms[i].perm,
+                               stream_perms[i].presorted, T->shard_rank, T->shard_count,
+                               StreamTiling(), &T->streams[i]);
+    }
     if (rc != SPLATT_SUCCESS) { splatt_b200_tensor_free(T); return rc; }
     if (bo.verbosity >= SPLATT_VERBOSITY_MAX) {
       const FiberStream & s = T->streams[i];
@@ -614,6 +616,37 @@ void splatt_b200_csf_free(splatt_csf * csf, int csf_alloc) {
     free(csf[c].pt);
   }
   free(csf);
+}
+
+int splatt_b200_cta_tiling(int nmodes, uint64_t const * dims, int const * perm,
+                           uint64_t nnz_local, int shard_count, int root_only, int num_sms,
+                           int force, uint32_t * tile_rows, uint32_t * acc_rows) {
+  if (tile_rows) *tile_rows = 0;
+  if (acc_rows) *acc_rows = 0;
+  if (!dims || !perm || !tile_rows || !acc_rows || nmodes != 3 || num_sms < 1 || nnz_local == 0)
+    return 0;
+  const uint64_t root_dim = dims[perm[0]], leaf_dim = dims[perm[nmodes - 1]];
+  // root rows one range (1 / num_sms of the records) spans if roots are spread evenly, plus
+  // a margin; the build checks the real spans and drops the tiling when one does not fit
+  const uint64_t slices = std::max<uint64_t>(1, std::min(root_dim, nnz_local));
+  uint64_t acc = (root_dim + num_sms - 1) / num_sms;
+  acc += acc / 4 + 8;
+  if (force) acc = std::max<uint64_t>(acc, std::min<uint64_t>(root_dim, 256));
+  if (acc > 0xffffu) return 0;
+  const uint32_t rows = spb200_tiled_rows_for((uint32_t)acc);
+  if (force) {
+    if (rows < 1) return 0;
+  } else {
+    const double reuse = (double)nnz_local / num_sms / (double)std::max<uint64_t>(leaf_dim, 1);
+    const uint64_t ntiles = (leaf_dim + std::max<uint32_t>(rows, 1) - 1) / std::max<uint32_t>(rows, 1);
+    const double per_piece = (double)nnz_local / (double)slices / (double)ntiles;
+    if (shard_count > 1 || !root_only || rows < 16 || leaf_dim <= rows || reuse < 3.0 ||
+        nnz_local < (uint64_t)num_sms * 4096 || per_piece < SPB200_MIN_NNZ_PER_PIECE)
+      return 0;
+  }
+  *tile_rows = rows;
+  *acc_rows = (uint32_t)acc;
+  return 1;
 }
 
 int splatt_b200_level_orders(uint64_t const * dims, int nmodes, int csf_alloc, int * perms,

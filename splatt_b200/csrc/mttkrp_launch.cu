@@ -100,18 +100,16 @@ int spb200_launch_mttkrp(const FiberStream & s, int kind, int outdepth, int ncol
   }
   if (s.nrec == 0 && !(multicast_out && sync)) return SPLATT_SUCCESS;
 
-  // leaf factor staged in shared memory (CTA-tiled stream, 3-mode root, one column pass)
-  if (!multicast_out && col_begin == 0 && col_end == rpad_all &&
-      spb200_tiled_applicable(s, kind, ncolumns, ldm)) {
+  // leaf factor staged in shared memory (CTA-tiled stream, 3-mode root)
+  if (!multicast_out && spb200_tiled_applicable(s, kind)) {
     static int use_tiled = -1;
     if (use_tiled < 0) {
       const char * e = getenv("SPLATT_B200_TILED_KERNEL");
       use_tiled = (e && atoi(e) == 0) ? 0 : 1;
     }
     if (use_tiled)
-      return spb200_launch_tiled_root3(s, ncolumns, ldm, s.leaf_rows,
-                                       d_mats_by_mode[s.perm[2]], d_mats_by_mode[s.perm[1]], d_out,
-                                       stream);
+      return spb200_launch_tiled_root3(s, ldm, col_begin, col_end, d_mats_by_mode[s.perm[2]],
+                                       d_mats_by_mode[s.perm[1]], d_out, stream);
   }
 
   MttkrpArgs a;

@@ -6,37 +6,52 @@
 // half of those gathers can be served from shared memory instead:
 //
 //   * the stream is built "CTA-tiled" (stream_build.cu): the records of CTA r's range
-//     are regrouped by leaf tile, seg_off[r * ntiles + t] marks the segments;
+//     are regrouped by leaf tile, seg_off[r * ntiles + t] marks the segments, and
+//     rroot[2r], rroot[2r + 1] bound the root rows the range touches;
 //   * one persistent CTA per SM walks its range tile by tile; a producer warp streams
 //     the leaf-factor tiles (TMA bulk copies, double buffered, mbarrier full/empty);
 //   * consumer warps stage their records through a private TMA ring as before, read
 //     the leaf row from the tile (LDS.128) and gather only the parent row from L2;
-//   * slice / sub-range ends reduce into the output with red.global.add.f64.
+//   * slice / sub-range ends add into a shared-memory block holding the range's root
+//     rows; at the end interior rows are stored, and only the first and last row (which
+//     the neighbouring ranges may share) are reduced into the output.
 //
-// Same results as the generic kernel (linearity); chosen by spb200_launch_mttkrp when the
-// stream carries the tiling and the launch parameters fit.
+// Columns are processed in slabs of kSlab: the tile and the accumulator hold one slab, and
+// the CTA re-walks its records once per slab, all inside one launch.  Same results as the
+// generic kernel (linearity); chosen by spb200_launch_mttkrp whenever the stream carries the
+// tiling.
 #include "mttkrp_kernels.cuh"
 
 namespace spb200 {
 
-constexpr int kTW  = 24;          // consumer warps per CTA (+ 1 producer warp)
-constexpr int kTRS = 96;          // records per warp per staging round
-constexpr int kTB  = 4;           // records whose gathers are issued together
+constexpr int kTW   = 24;         // consumer warps per CTA (+ 1 producer warp)
+constexpr int kTRS  = 96;         // records per warp per staging round
+constexpr int kTB   = 4;          // records whose gathers are issued together
+constexpr int kSlab = 32;         // columns held in shared memory at a time
 
 struct TiledArgs {
   const SpRec *    rec;
   const uint32_t * rootid;
   const uint32_t * seg_off;       // this grid's ranges: [gridDim.x * ntiles + 1]
+  const uint32_t * rroot;         // [2 * gridDim.x] first / last root row of every range
   const double *   leaf;
   const double *   parent;
   double *         out;
   uint32_t         ntiles, tile_rows, leaf_rows;
-  uint32_t         tile_bytes;    // bytes reserved per tile buffer (tile_rows * pitch)
-  int              ldm, ncols, col0;
+  uint32_t         tile_bytes;    // bytes reserved per tile buffer (tile_rows * kSlab * 8)
+  uint32_t         tpitch;        // bytes per row of a staged tile
+  uint32_t         acc_rows;      // rows of the shared accumulator
+  int              ldm, col0, col_end;
+  int              whole;         // 1: one slab and ldm <= kSlab: a tile is one contiguous copy
 };
 
 __device__ __forceinline__ void mbar_wait(uint64_t * bar, uint32_t parity) {
   while (!mbar_try_wait(bar, parity)) {}
+}
+
+// barrier of the consumer warps only (the producer warp has left)
+__device__ __forceinline__ void consumers_sync() {
+  asm volatile("bar.sync 1, %0;" ::"n"(kTW * 32) : "memory");
 }
 
 template <int L>
@@ -45,8 +60,9 @@ __global__ void __launch_bounds__((kTW + 1) * 32, 1) mttkrp_tiled_root3(const Ti
   constexpr int NG = kTW * G;     // lane groups per CTA
 
   extern __shared__ __align__(128) unsigned char smem[];
-  unsigned char * tiles = smem;                                   // 2 x tile_bytes
-  SpRec *    ring = reinterpret_cast<SpRec *>(smem + 2 * a.tile_bytes);       // [kTW][2][kTRS]
+  unsigned char * tiles = smem;                                              // 2 x tile_bytes
+  double *   accs = reinterpret_cast<double *>(smem + 2 * a.tile_bytes);    // [acc_rows][kSlab]
+  SpRec *    ring = reinterpret_cast<SpRec *>(accs + static_cast<size_t>(a.acc_rows) * kSlab);
   uint64_t * bars = reinterpret_cast<uint64_t *>(ring + kTW * 2 * kTRS);
   uint64_t * tile_full  = bars;            // [2]
   uint64_t * tile_empty = bars + 2;        // [2]
@@ -56,8 +72,13 @@ __global__ void __launch_bounds__((kTW + 1) * 32, 1) mttkrp_tiled_root3(const Ti
   const int      lane  = threadIdx.x & 31;
   const uint32_t pitch = static_cast<uint32_t>(a.ldm) * 8u;
   const uint32_t NT    = a.ntiles;
+  const uint32_t NS    = static_cast<uint32_t>(a.col_end - a.col0 + kSlab - 1) / kSlab;
   const uint32_t * so  = a.seg_off + static_cast<size_t>(blockIdx.x) * NT;
+  const uint32_t r_lo  = a.rroot[2 * blockIdx.x];
+  const uint32_t nrows = (a.rroot[2 * blockIdx.x + 1] >= r_lo) ? a.rroot[2 * blockIdx.x + 1] - r_lo + 1 : 0u;
 
+  for (uint32_t i = threadIdx.x; i < nrows * (kSlab / 2); i += blockDim.x)
+    reinterpret_cast<double2 *>(accs)[i] = make_double2(0.0, 0.0);
   if (threadIdx.x == 0) {
     for (int b = 0; b < 2; ++b) { mbar_init(&tile_full[b], 1); mbar_init(&tile_empty[b], kTW); }
     for (int w = 0; w < kTW * 2; ++w) mbar_init(&rec_full[w], 1);
@@ -73,18 +94,30 @@ __global__ void __launch_bounds__((kTW + 1) * 32, 1) mttkrp_tiled_root3(const Ti
 
   // ------------------------------------------------------------------ producer warp
   if (warp == kTW) {
-    if (lane == 0) {
-      for (uint32_t t = 0; t < NT; ++t) {
-        const uint32_t b = t & 1u;
-        if (t >= 2) mbar_wait(&tile_empty[b], ((t - 2) >> 1) & 1u);   // all warps left tile t-2
-        const uint32_t bytes = tile_rows_of(t) * pitch;
-        mbar_arrive_expect_tx(&tile_full[b], bytes);
-        const char * src = reinterpret_cast<const char *>(a.leaf) +
-                           static_cast<size_t>(t) * a.tile_rows * pitch;
-        // bulk copies of at most 32 KB each
-        for (uint32_t off = 0; off < bytes; off += 32768u)
-          tma_bulk_g2s(tiles + b * a.tile_bytes + off, src + off, min(32768u, bytes - off),
-                       &tile_full[b]);
+    for (uint32_t gt = 0; gt < NS * NT; ++gt) {
+      const uint32_t t = gt % NT, b = gt & 1u;
+      if (gt >= 2) mbar_wait(&tile_empty[b], ((gt - 2) >> 1) & 1u);   // all warps left tile gt-2
+      const uint32_t rows = tile_rows_of(t);
+      unsigned char * dst = tiles + b * a.tile_bytes;
+      if (a.whole) {
+        if (lane == 0) {
+          const uint32_t bytes = rows * pitch;
+          mbar_arrive_expect_tx(&tile_full[b], bytes);
+          const char * src = reinterpret_cast<const char *>(a.leaf) +
+                             static_cast<size_t>(t) * a.tile_rows * pitch;
+          // bulk copies of at most 32 KB each
+          for (uint32_t off = 0; off < bytes; off += 32768u)
+            tma_bulk_g2s(dst + off, src + off, min(32768u, bytes - off), &tile_full[b]);
+        }
+      } else {
+        // one slab of every row: a strided block, one bulk copy per row spread over the lanes
+        const int      sc0 = a.col0 + static_cast<int>(gt / NT) * kSlab;
+        const uint32_t sb  = static_cast<uint32_t>(min(kSlab, a.col_end - sc0)) * 8u;
+        if (lane == 0) mbar_arrive_expect_tx(&tile_full[b], rows * sb);
+        __syncwarp();
+        const double * src = a.leaf + static_cast<size_t>(t) * a.tile_rows * a.ldm + sc0;
+        for (uint32_t i = lane; i < rows; i += 32)
+          tma_bulk_g2s(dst + i * a.tpitch, src + static_cast<size_t>(i) * a.ldm, sb, &tile_full[b]);
       }
     }
     return;
@@ -93,12 +126,7 @@ __global__ void __launch_bounds__((kTW + 1) * 32, 1) mttkrp_tiled_root3(const Ti
   // ------------------------------------------------------------------ consumer warps
   const int  grp    = lane / L;
   const int  gl     = lane % L;
-  const bool act    = (2 * gl) < a.ncols;
   const bool leader = (gl == 0);
-  const int  colx   = act ? (a.col0 + 2 * gl) : a.col0;
-  const char * pbase = reinterpret_cast<const char *>(a.parent + colx);
-  char *       obase = reinterpret_cast<char *>(a.out + colx);
-  const uint32_t tcol = static_cast<uint32_t>(colx) * 8u;      // byte offset of this lane's columns
   SpRec *    myring = ring + warp * 2 * kTRS;
   uint64_t * mybars = rec_full + warp * 2;
 
@@ -109,12 +137,13 @@ __global__ void __launch_bounds__((kTW + 1) * 32, 1) mttkrp_tiled_root3(const Ti
     hi = s0 + static_cast<uint32_t>(static_cast<unsigned long long>(g1) * len / NG);
   };
 
-  // issue side: rounds are enumerated tile-major, at least one (possibly empty) per tile
+  // issue side: rounds are enumerated slab-major, then tile-major, at least one (possibly
+  // empty) per tile
   uint32_t it = 0, ioff = 0, ij = 0;
   auto issue_next = [&]() {
-    if (it >= NT) return;
+    if (it >= NS * NT) return;
     uint32_t ws, we;
-    part(it, warp * G, (warp + 1) * G, ws, we);
+    part(it % NT, warp * G, (warp + 1) * G, ws, we);
     const uint32_t rs  = ws + ioff;
     const uint32_t cnt = (rs < we) ? min(static_cast<uint32_t>(kTRS), we - rs) : 0u;
     if (lane == 0) {
@@ -138,123 +167,153 @@ __global__ void __launch_bounds__((kTW + 1) * 32, 1) mttkrp_tiled_root3(const Ti
   double2 acc1 = zero2, acc0 = zero2;      // fiber / slice partial sums
   uint32_t j = 0;                          // rounds consumed
 
-  for (uint32_t t = 0; t < NT; ++t) {
-    mbar_wait(&tile_full[t & 1u], (t >> 1) & 1u);
-    const unsigned char * tile = tiles + (t & 1u) * a.tile_bytes + tcol;
-    const uint32_t kbase = t * a.tile_rows;
-    uint32_t ws, we, gs, ge;
-    part(t, warp * G, (warp + 1) * G, ws, we);
-    part(t, warp * G + grp, warp * G + grp + 1, gs, ge);
-    const uint32_t nr = (we > ws) ? (we - ws + kTRS - 1) / kTRS : 1u;
-    for (uint32_t i = 0; i < nr; ++i, ++j) {
-      mbar_wait(&mybars[j & 1u], (j >> 1) & 1u);
-      SpRec *        buf = myring + (j & 1u) * kTRS;
-      const uint32_t rs  = ws + i * kTRS;
-      const uint32_t re  = min(we, rs + kTRS);
-      const uint32_t lo  = max(gs, rs), hi = min(ge, re);
-      // the group's last record of this tile closes the slice (sub-range boundary)
-      if (leader && hi > lo && hi == ge)
-        buf[hi - 1 - rs].aux = (buf[hi - 1 - rs].aux & SPB200_IDX_MASK) | (2u << SPB200_IDX_BITS);
-      __syncwarp();
-      if (act && hi > lo) {
-        uint32_t n = lo;
-        for (; n + kTB <= hi; n += kTB) {
-          uint4   q[kTB];
-          double2 b[kTB], r[kTB];
-          uint32_t any = 0;
-#pragma unroll
-          for (int u = 0; u < kTB; ++u) {
-            q[u] = *reinterpret_cast<const uint4 *>(&buf[n + u - rs]);
-            any |= q[u].w;
-          }
-#pragma unroll
-          for (int u = 0; u < kTB; ++u)
-            if (q[u].w >> SPB200_IDX_BITS) r[u] = ld_row_na(pbase, q[u].w & SPB200_IDX_MASK, pitch);
-#pragma unroll
-          for (int u = 0; u < kTB; ++u)
-            b[u] = *reinterpret_cast<const double2 *>(tile + static_cast<size_t>(q[u].z - kbase) * pitch);
-          if ((any >> (SPB200_IDX_BITS + 1)) == 0) {
+  for (uint32_t s = 0; s < NS; ++s) {
+    const int    sc0  = a.col0 + static_cast<int>(s) * kSlab;
+    const int    sw   = min(kSlab, a.col_end - sc0);
+    const bool   act  = (2 * gl) < sw;
+    const int    c2   = act ? 2 * gl : 0;                    // this lane's columns in the slab
+    const char * pbase = reinterpret_cast<const char *>(a.parent + sc0 + c2);
+    const uint32_t tcol = static_cast<uint32_t>((a.whole ? sc0 : 0) + c2) * 8u;
+    double *     abase = accs + c2;
+    auto flush = [&](uint32_t n) {                           // the slice closed: into smem
+      double * p = abase + static_cast<size_t>(__ldg(&a.rootid[n]) - r_lo) * kSlab;
+      atomicAdd(p, acc0.x);
+      atomicAdd(p + 1, acc0.y);
+      acc0 = zero2;
+    };
+
+    for (uint32_t t = 0; t < NT; ++t) {
+      const uint32_t gt = s * NT + t;
+      mbar_wait(&tile_full[gt & 1u], (gt >> 1) & 1u);
+      const unsigned char * tile = tiles + (gt & 1u) * a.tile_bytes + tcol;
+      const uint32_t kbase = t * a.tile_rows;
+      uint32_t ws, we, gs, ge;
+      part(t, warp * G, (warp + 1) * G, ws, we);
+      part(t, warp * G + grp, warp * G + grp + 1, gs, ge);
+      const uint32_t nr = (we > ws) ? (we - ws + kTRS - 1) / kTRS : 1u;
+      for (uint32_t i = 0; i < nr; ++i, ++j) {
+        mbar_wait(&mybars[j & 1u], (j >> 1) & 1u);
+        SpRec *        buf = myring + (j & 1u) * kTRS;
+        const uint32_t rs  = ws + i * kTRS;
+        const uint32_t re  = min(we, rs + kTRS);
+        const uint32_t lo  = max(gs, rs), hi = min(ge, re);
+        // the group's last record of this tile closes the slice (sub-range boundary)
+        if (leader && hi > lo && hi == ge)
+          buf[hi - 1 - rs].aux = (buf[hi - 1 - rs].aux & SPB200_IDX_MASK) | (2u << SPB200_IDX_BITS);
+        __syncwarp();
+        if (act && hi > lo) {
+          uint32_t n = lo;
+          for (; n + kTB <= hi; n += kTB) {
+            uint4   q[kTB];
+            double2 b[kTB], r[kTB];
+            uint32_t any = 0;
 #pragma unroll
             for (int u = 0; u < kTB; ++u) {
-              const double v = __hiloint2double(static_cast<int>(q[u].y), static_cast<int>(q[u].x));
-              acc1           = fma2(v, b[u], acc1);
-              if (q[u].w >> SPB200_IDX_BITS) { acc0 = fma2(acc1, r[u], acc0); acc1 = zero2; }
+              q[u] = *reinterpret_cast<const uint4 *>(&buf[n + u - rs]);
+              any |= q[u].w;
             }
-          } else {
 #pragma unroll
-            for (int u = 0; u < kTB; ++u) {
-              const double   v = __hiloint2double(static_cast<int>(q[u].y), static_cast<int>(q[u].x));
-              const uint32_t c = q[u].w >> SPB200_IDX_BITS;
-              acc1             = fma2(v, b[u], acc1);
-              if (c) {
-                acc0 = fma2(acc1, r[u], acc0);
-                acc1 = zero2;
-                if (c >= 2) {
-                  red_row(obase, __ldg(&a.rootid[n + u]), pitch, acc0);
-                  acc0 = zero2;
+            for (int u = 0; u < kTB; ++u)
+              if (q[u].w >> SPB200_IDX_BITS) r[u] = ld_row_na(pbase, q[u].w & SPB200_IDX_MASK, pitch);
+#pragma unroll
+            for (int u = 0; u < kTB; ++u)
+              b[u] = *reinterpret_cast<const double2 *>(tile + static_cast<size_t>(q[u].z - kbase) * a.tpitch);
+            if ((any >> (SPB200_IDX_BITS + 1)) == 0) {
+#pragma unroll
+              for (int u = 0; u < kTB; ++u) {
+                const double v = __hiloint2double(static_cast<int>(q[u].y), static_cast<int>(q[u].x));
+                acc1           = fma2(v, b[u], acc1);
+                if (q[u].w >> SPB200_IDX_BITS) { acc0 = fma2(acc1, r[u], acc0); acc1 = zero2; }
+              }
+            } else {
+#pragma unroll
+              for (int u = 0; u < kTB; ++u) {
+                const double   v = __hiloint2double(static_cast<int>(q[u].y), static_cast<int>(q[u].x));
+                const uint32_t c = q[u].w >> SPB200_IDX_BITS;
+                acc1             = fma2(v, b[u], acc1);
+                if (c) {
+                  acc0 = fma2(acc1, r[u], acc0);
+                  acc1 = zero2;
+                  if (c >= 2) flush(n + u);
                 }
               }
             }
           }
-        }
-        for (; n < hi; ++n) {
-          const uint4    q = *reinterpret_cast<const uint4 *>(&buf[n - rs]);
-          const double   v = __hiloint2double(static_cast<int>(q.y), static_cast<int>(q.x));
-          const uint32_t c = q.w >> SPB200_IDX_BITS;
-          const double2  b = *reinterpret_cast<const double2 *>(tile + static_cast<size_t>(q.z - kbase) * pitch);
-          acc1             = fma2(v, b, acc1);
-          if (c) {
-            acc0 = fma2(acc1, ld_row_na(pbase, q.w & SPB200_IDX_MASK, pitch), acc0);
-            acc1 = zero2;
-            if (c >= 2) {
-              red_row(obase, __ldg(&a.rootid[n]), pitch, acc0);
-              acc0 = zero2;
+          for (; n < hi; ++n) {
+            const uint4    q = *reinterpret_cast<const uint4 *>(&buf[n - rs]);
+            const double   v = __hiloint2double(static_cast<int>(q.y), static_cast<int>(q.x));
+            const uint32_t c = q.w >> SPB200_IDX_BITS;
+            const double2  b = *reinterpret_cast<const double2 *>(tile + static_cast<size_t>(q.z - kbase) * a.tpitch);
+            acc1             = fma2(v, b, acc1);
+            if (c) {
+              acc0 = fma2(acc1, ld_row_na(pbase, q.w & SPB200_IDX_MASK, pitch), acc0);
+              acc1 = zero2;
+              if (c >= 2) flush(n);
             }
           }
         }
+        __syncwarp();
+        issue_next();        // refill the stage just consumed with round j + 2
       }
       __syncwarp();
-      issue_next();        // refill the stage just consumed with round j + 2
+      if (lane == 0) mbar_arrive(&tile_empty[gt & 1u]);    // this warp is done with tile gt
     }
-    __syncwarp();
-    if (lane == 0) mbar_arrive(&tile_empty[t & 1u]);    // this warp is done with tile t
+
+    // the slab is complete: interior rows belong to this range alone and are stored; the
+    // first and last row may be shared with the neighbouring ranges and are reduced
+    consumers_sync();
+    const uint32_t pairs = static_cast<uint32_t>(sw) / 2u;
+    for (uint32_t i = threadIdx.x; i < nrows * pairs; i += kTW * 32) {
+      const uint32_t row = i / pairs, c = 2u * (i % pairs);
+      double2 *      src = reinterpret_cast<double2 *>(accs + static_cast<size_t>(row) * kSlab + c);
+      const double2  v   = *src;
+      *src = zero2;
+      double * dst = a.out + static_cast<size_t>(r_lo + row) * a.ldm + sc0 + c;
+      if (row == 0 || row + 1 == nrows) {
+        atomicAdd(dst, v.x);
+        atomicAdd(dst + 1, v.y);
+      } else {
+        *reinterpret_cast<double2 *>(dst) = v;
+      }
+    }
+    consumers_sync();
   }
 }
 
 }  // namespace spb200
 
-// smem the kernel needs for a given tile size
-static size_t tiled_smem_bytes(uint32_t tile_bytes) {
-  return 2 * (size_t)tile_bytes + sizeof(SpRec) * spb200::kTW * 2 * spb200::kTRS +
-         sizeof(uint64_t) * (4 + 2 * spb200::kTW) + 128;
+// smem the kernel needs for a tile of `tile_rows` and an accumulator of `acc_rows` rows
+static size_t tiled_smem_bytes(uint32_t tile_rows, uint32_t acc_rows) {
+  using namespace spb200;
+  return (2 * (size_t)tile_rows + acc_rows) * kSlab * 8 + sizeof(SpRec) * kTW * 2 * kTRS +
+         sizeof(uint64_t) * (4 + 2 * kTW) + 128;
 }
 
-uint32_t spb200_tiled_rows_for(int ncolumns) {
-  const size_t pitch = (size_t)(ncolumns + (ncolumns & 1)) * 8;
-  const size_t fixed = tiled_smem_bytes(0);
-  const size_t avail = (227 * 1024 - fixed) / 2;
-  return (uint32_t)(avail / pitch);
+uint32_t spb200_tiled_rows_for(uint32_t acc_rows) {
+  const size_t fixed = tiled_smem_bytes(0, acc_rows);
+  if (fixed >= 227 * 1024) return 0;
+  return (uint32_t)((227 * 1024 - fixed) / 2 / (spb200::kSlab * 8));
 }
 
-bool spb200_tiled_applicable(const FiberStream & s, int kind, int ncolumns, int ldm) {
-  if (s.nmodes != 3 || kind != SPB200_KIND_ROOT || !s.seg_off || !s.rootid || s.ntiles == 0) return false;
-  const int rpad = ncolumns + (ncolumns & 1);
-  if (rpad > 64) return false;                       // single column pass only
-  const size_t tile_bytes = (size_t)s.ktile_rows * ldm * 8;
-  return tiled_smem_bytes((uint32_t)tile_bytes) <= 227 * 1024;
+bool spb200_tiled_applicable(const FiberStream & s, int kind) {
+  return s.nmodes == 3 && kind == SPB200_KIND_ROOT && s.seg_off && s.rootid && s.rroot &&
+         s.ntiles > 0 && tiled_smem_bytes(s.ktile_rows, s.acc_rows) <= 227 * 1024;
 }
 
-int spb200_launch_tiled_root3(const FiberStream & s, int ncolumns, int ldm, uint64_t leaf_rows,
-                                   const double * leaf, const double * parent, double * d_out,
-                                   cudaStream_t stream) {
+int spb200_launch_tiled_root3(const FiberStream & s, int ldm, int col_begin, int col_end,
+                              const double * leaf, const double * parent, double * d_out,
+                              cudaStream_t stream) {
   using namespace spb200;
   TiledArgs a;
-  a.rec = s.rec; a.rootid = s.rootid; a.seg_off = s.seg_off;
+  a.rec = s.rec; a.rootid = s.rootid; a.seg_off = s.seg_off; a.rroot = s.rroot;
   a.leaf = leaf; a.parent = parent; a.out = d_out;
-  a.ntiles = s.ntiles; a.tile_rows = s.ktile_rows; a.leaf_rows = (uint32_t)leaf_rows;
-  a.ldm = ldm; a.col0 = 0; a.ncols = ncolumns + (ncolumns & 1);
-  a.tile_bytes = s.ktile_rows * (uint32_t)ldm * 8u;
-  const size_t smem = tiled_smem_bytes(a.tile_bytes);
+  a.ntiles = s.ntiles; a.tile_rows = s.ktile_rows; a.leaf_rows = (uint32_t)s.leaf_rows;
+  a.acc_rows = s.acc_rows;
+  a.ldm = ldm; a.col0 = col_begin; a.col_end = col_end;
+  a.whole = (col_end - col_begin <= kSlab && ldm <= kSlab) ? 1 : 0;
+  a.tile_bytes = s.ktile_rows * kSlab * 8u;
+  a.tpitch = a.whole ? (uint32_t)ldm * 8u : kSlab * 8u;
+  const size_t smem = tiled_smem_bytes(s.ktile_rows, s.acc_rows);
   const int threads = (kTW + 1) * 32;
   const unsigned grid = s.kranges;
 #define SPB200_TILED_LAUNCH(LL)                                                                   \
@@ -269,10 +328,10 @@ int spb200_launch_tiled_root3(const FiberStream & s, int ncolumns, int ldm, uint
     }                                                                                             \
     mttkrp_tiled_root3<LL><<<grid, threads, smem, stream>>>(a);                                   \
   } while (0)
-  if (a.ncols <= 8) SPB200_TILED_LAUNCH(4);
-  else if (a.ncols <= 16) SPB200_TILED_LAUNCH(8);
-  else if (a.ncols <= 32) SPB200_TILED_LAUNCH(16);
-  else SPB200_TILED_LAUNCH(32);
+  const int width = col_end - col_begin;
+  if (width <= 8) SPB200_TILED_LAUNCH(4);
+  else if (width <= 16) SPB200_TILED_LAUNCH(8);
+  else SPB200_TILED_LAUNCH(16);
 #undef SPB200_TILED_LAUNCH
   spb200_count_launches(1);
   SPB200_CUDA_OK(cudaGetLastError());

@@ -266,6 +266,29 @@ __global__ void k_seg_offsets(const uint32_t * __restrict__ seg, uint64_t n, uin
   for (uint32_t k = lo; k <= hi; ++k) seg_off[k] = (uint32_t)i;
 }
 
+// rroot[2r], rroot[2r + 1] = least / greatest root index of the records of range r
+// (seg_off[r * ntiles] .. seg_off[(r + 1) * ntiles]); an empty range gets 1, 0.
+__global__ void k_range_roots(const uint32_t * __restrict__ rootid,
+                              const uint32_t * __restrict__ seg_off, uint32_t ntiles,
+                              uint32_t * __restrict__ rroot) {
+  __shared__ uint32_t lo, hi;
+  if (threadIdx.x == 0) { lo = 0xffffffffu; hi = 0u; }
+  __syncthreads();
+  const uint32_t b = seg_off[(size_t)blockIdx.x * ntiles], e = seg_off[(size_t)(blockIdx.x + 1) * ntiles];
+  uint32_t l = 0xffffffffu, h = 0u;
+  for (uint32_t i = b + threadIdx.x; i < e; i += blockDim.x) {
+    l = min(l, rootid[i]);
+    h = max(h, rootid[i]);
+  }
+  atomicMin(&lo, l);
+  atomicMax(&hi, h);
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    rroot[2 * blockIdx.x]     = (b < e) ? lo : 1u;
+    rroot[2 * blockIdx.x + 1] = (b < e) ? hi : 0u;
+  }
+}
+
 __global__ void k_offset_iota(uint32_t * o, uint64_t n0, uint64_t n) {
   uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
   if (i < n) o[i] = (uint32_t)(n0 + i);
@@ -332,6 +355,7 @@ void spb200_free_stream(FiberStream * s) {
   if (s->rec) cudaFree(s->rec);
   if (s->seg_off) cudaFree(s->seg_off);
   if (s->rootid) cudaFree(s->rootid);
+  if (s->rroot) cudaFree(s->rroot);
   for (int l = 0; l < SPB200_MAXN; ++l)
     if (s->up[l]) cudaFree(s->up[l]);
   if (s->desc) cudaFree(s->desc);
@@ -390,18 +414,26 @@ int spb200_build_stream(int N, const uint64_t * dims, uint64_t nnz,
   if (tiled && tiling.cta) {
     const uint32_t ntiles = (uint32_t)((dims[perm[N - 1]] + tiling.tile_rows - 1) / tiling.tile_rows);
     const uint32_t nkeys = tiling.nranges * ntiles;
-    void * so = nullptr; void * ri = nullptr;
+    void * so = nullptr; void * ri = nullptr; void * rr = nullptr;
     if (cudaMalloc(&so, ((size_t)nkeys + 1) * 4) != cudaSuccess ||
-        cudaMalloc(&ri, std::max<uint64_t>(nrec, 1) * 4) != cudaSuccess) {
+        cudaMalloc(&ri, std::max<uint64_t>(nrec, 1) * 4) != cudaSuccess ||
+        cudaMalloc(&rr, (size_t)tiling.nranges * 2 * 4) != cudaSuccess) {
       if (so) cudaFree(so);
+      if (ri) cudaFree(ri);
       return SPLATT_ERROR_NOMEMORY;
     }
     out->seg_off = static_cast<uint32_t *>(so);
     out->rootid = static_cast<uint32_t *>(ri);
+    out->rroot = static_cast<uint32_t *>(rr);
     out->ntiles = ntiles;
     k_seg_offsets<<<nblk(nrec + 1), 256>>>(seg.as<uint32_t>(), nrec, nkeys, out->seg_off);
     CK(cudaMemcpy(out->rootid, sc.sidx[0].as<uint32_t>(), nrec * 4, cudaMemcpyDeviceToDevice));
-    held += ((size_t)nkeys + 1) * 4 + nrec * 4;
+    k_range_roots<<<tiling.nranges, 256>>>(out->rootid, out->seg_off, ntiles, out->rroot);
+    std::vector<uint32_t> rh((size_t)tiling.nranges * 2);
+    CK(cudaMemcpy(rh.data(), out->rroot, rh.size() * 4, cudaMemcpyDeviceToHost));
+    for (uint32_t r = 0; r < tiling.nranges; ++r)
+      if (rh[2 * r + 1] >= rh[2 * r]) out->acc_rows = std::max(out->acc_rows, rh[2 * r + 1] - rh[2 * r] + 1);
+    held += ((size_t)nkeys + 1) * 4 + nrec * 4 + rh.size() * 4;
   }
   DevBuf flag, nid, tmp, desc;
   CK(flag.alloc(nrec * 4));
