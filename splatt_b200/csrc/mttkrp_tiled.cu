@@ -8,10 +8,11 @@
 //   * the stream is built "CTA-tiled" (stream_build.cu): the records of CTA r's range
 //     are regrouped by leaf tile, seg_off[r * ntiles + t] marks the segments, and
 //     rroot[2r], rroot[2r + 1] bound the root rows the range touches;
-//   * one persistent CTA per SM walks its range tile by tile; a producer warp streams
-//     the leaf-factor tiles (TMA bulk copies, double buffered, mbarrier full/empty);
-//   * consumer warps stage their records through a private TMA ring as before, read
-//     the leaf row from the tile (LDS.128) and gather only the parent row from L2;
+//   * one persistent CTA per SM walks its range tile by tile; the leaf-factor tiles are
+//     streamed in with TMA bulk copies, double buffered (mbarrier full, a counter of the
+//     warps done with a buffer);
+//   * every warp stages its records through a private TMA ring, reads the leaf row from
+//     the tile (LDS.128) and gathers only the parent row from L2;
 //   * slice / sub-range ends add into a shared-memory block holding the range's root
 //     rows; at the end interior rows are stored, and only the first and last row (which
 //     the neighbouring ranges may share) are reduced into the output.
@@ -24,7 +25,7 @@
 
 namespace spb200 {
 
-constexpr int kTW   = 24;         // consumer warps per CTA (+ 1 producer warp)
+constexpr int kTW   = 24;         // warps per CTA, all of them consuming records
 constexpr int kTRS  = 96;         // records per warp per staging round
 constexpr int kTB   = 4;          // records whose gathers are issued together
 constexpr int kSlab = 32;         // columns held in shared memory at a time
@@ -49,13 +50,20 @@ __device__ __forceinline__ void mbar_wait(uint64_t * bar, uint32_t parity) {
   while (!mbar_try_wait(bar, parity)) {}
 }
 
-// barrier of the consumer warps only (the producer warp has left)
-__device__ __forceinline__ void consumers_sync() {
-  asm volatile("bar.sync 1, %0;" ::"n"(kTW * 32) : "memory");
+// shared-memory load by 32-bit address (volatile: stays after the mbarrier wait that guards it)
+__device__ __forceinline__ double2 lds_f64x2(uint32_t addr) {
+  double2 r;
+  asm volatile("ld.shared.v2.f64 {%0, %1}, [%2];" : "=d"(r.x), "=d"(r.y) : "r"(addr));
+  return r;
 }
 
+// Every warp consumes records; there is no separate producer warp.  A 25th warp would cap
+// every thread at 72 registers instead of 80 and the batch loop spilled more (bench.py's
+// headline tensor, H100 80GB HBM3 at 700 W: 0.52 ms per mode with a producer warp, 0.48 ms
+// with this layout).  Leaf tiles are double buffered; the last warp to finish tile gt loads
+// tile gt + 2 into the buffer gt leaves.
 template <int L>
-__global__ void __launch_bounds__((kTW + 1) * 32, 1) mttkrp_tiled_root3(const TiledArgs a) {
+__global__ void __launch_bounds__(kTW * 32, 1) mttkrp_tiled_root3(const TiledArgs a) {
   constexpr int G  = 32 / L;
   constexpr int NG = kTW * G;     // lane groups per CTA
 
@@ -64,9 +72,9 @@ __global__ void __launch_bounds__((kTW + 1) * 32, 1) mttkrp_tiled_root3(const Ti
   double *   accs = reinterpret_cast<double *>(smem + 2 * a.tile_bytes);    // [acc_rows][kSlab]
   SpRec *    ring = reinterpret_cast<SpRec *>(accs + static_cast<size_t>(a.acc_rows) * kSlab);
   uint64_t * bars = reinterpret_cast<uint64_t *>(ring + kTW * 2 * kTRS);
-  uint64_t * tile_full  = bars;            // [2]
-  uint64_t * tile_empty = bars + 2;        // [2]
-  uint64_t * rec_full   = bars + 4;        // [kTW][2]
+  uint64_t * tile_full = bars;                                               // [2]
+  uint32_t * tile_left = reinterpret_cast<uint32_t *>(bars + 2);            // [2] warps done with a buffer
+  uint64_t * rec_full  = bars + 4;                                           // [kTW][2]
 
   const int      warp  = threadIdx.x >> 5;
   const int      lane  = threadIdx.x & 31;
@@ -75,55 +83,55 @@ __global__ void __launch_bounds__((kTW + 1) * 32, 1) mttkrp_tiled_root3(const Ti
   const uint32_t NS    = static_cast<uint32_t>(a.col_end - a.col0 + kSlab - 1) / kSlab;
   const uint32_t * so  = a.seg_off + static_cast<size_t>(blockIdx.x) * NT;
   const uint32_t r_lo  = a.rroot[2 * blockIdx.x];
-  const uint32_t nrows = (a.rroot[2 * blockIdx.x + 1] >= r_lo) ? a.rroot[2 * blockIdx.x + 1] - r_lo + 1 : 0u;
+  // root rows of this range; re-read where needed rather than held across the main loop
+  auto range_rows = [&]() {
+    const uint32_t r_hi = __ldg(&a.rroot[2 * blockIdx.x + 1]);
+    return (r_hi >= r_lo) ? r_hi - r_lo + 1 : 0u;
+  };
 
-  for (uint32_t i = threadIdx.x; i < nrows * (kSlab / 2); i += blockDim.x)
+  for (uint32_t i = threadIdx.x, nrows = range_rows(); i < nrows * (kSlab / 2); i += blockDim.x)
     reinterpret_cast<double2 *>(accs)[i] = make_double2(0.0, 0.0);
   if (threadIdx.x == 0) {
-    for (int b = 0; b < 2; ++b) { mbar_init(&tile_full[b], 1); mbar_init(&tile_empty[b], kTW); }
+    for (int b = 0; b < 2; ++b) { mbar_init(&tile_full[b], 1); tile_left[b] = 0; }
     for (int w = 0; w < kTW * 2; ++w) mbar_init(&rec_full[w], 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
   }
   __syncthreads();
 
-  auto tile_rows_of = [&](uint32_t t) {
-    const uint32_t first = t * a.tile_rows;
-    return min(a.tile_rows, a.leaf_rows - first);
-  };
-
-  // ------------------------------------------------------------------ producer warp
-  if (warp == kTW) {
-    for (uint32_t gt = 0; gt < NS * NT; ++gt) {
-      const uint32_t t = gt % NT, b = gt & 1u;
-      if (gt >= 2) mbar_wait(&tile_empty[b], ((gt - 2) >> 1) & 1u);   // all warps left tile gt-2
-      const uint32_t rows = tile_rows_of(t);
-      unsigned char * dst = tiles + b * a.tile_bytes;
-      if (a.whole) {
-        if (lane == 0) {
-          const uint32_t bytes = rows * pitch;
-          mbar_arrive_expect_tx(&tile_full[b], bytes);
-          const char * src = reinterpret_cast<const char *>(a.leaf) +
-                             static_cast<size_t>(t) * a.tile_rows * pitch;
-          // bulk copies of at most 32 KB each
-          for (uint32_t off = 0; off < bytes; off += 32768u)
-            tma_bulk_g2s(dst + off, src + off, min(32768u, bytes - off), &tile_full[b]);
-        }
-      } else {
-        // one slab of every row: a strided block, one bulk copy per row spread over the lanes
-        const int      sc0 = a.col0 + static_cast<int>(gt / NT) * kSlab;
-        const uint32_t sb  = static_cast<uint32_t>(min(kSlab, a.col_end - sc0)) * 8u;
-        if (lane == 0) mbar_arrive_expect_tx(&tile_full[b], rows * sb);
-        __syncwarp();
-        const double * src = a.leaf + static_cast<size_t>(t) * a.tile_rows * a.ldm + sc0;
-        for (uint32_t i = lane; i < rows; i += 32)
-          tma_bulk_g2s(dst + i * a.tpitch, src + static_cast<size_t>(i) * a.ldm, sb, &tile_full[b]);
+  // one warp loads tile gt (slab gt / NT, tile gt % NT) into buffer gt & 1
+  auto load_tile = [&](uint32_t gt) {
+    const uint32_t t = gt % NT, b = gt & 1u;
+    const uint32_t rows = min(a.tile_rows, a.leaf_rows - t * a.tile_rows);
+    unsigned char * dst = tiles + b * a.tile_bytes;
+    // generic-proxy reads of this buffer (the tile gt - 2) are ordered before the async writes
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    if (a.whole) {
+      if (lane == 0) {
+        const uint32_t bytes = rows * pitch;
+        mbar_arrive_expect_tx(&tile_full[b], bytes);
+        const char * src = reinterpret_cast<const char *>(a.leaf) +
+                           static_cast<size_t>(t) * a.tile_rows * pitch;
+        // bulk copies of at most 32 KB each
+        for (uint32_t off = 0; off < bytes; off += 32768u)
+          tma_bulk_g2s(dst + off, src + off, min(32768u, bytes - off), &tile_full[b]);
       }
+    } else {
+      // one slab of every row: a strided block, one bulk copy per row spread over the lanes
+      const int      sc0 = a.col0 + static_cast<int>(gt / NT) * kSlab;
+      const uint32_t sb  = static_cast<uint32_t>(min(kSlab, a.col_end - sc0)) * 8u;
+      if (lane == 0) mbar_arrive_expect_tx(&tile_full[b], rows * sb);
+      __syncwarp();
+      const double * src = a.leaf + static_cast<size_t>(t) * a.tile_rows * a.ldm + sc0;
+      for (uint32_t i = lane; i < rows; i += 32)
+        tma_bulk_g2s(dst + i * a.tpitch, src + static_cast<size_t>(i) * a.ldm, sb, &tile_full[b]);
     }
-    return;
+  };
+  if (warp == 0) {
+    load_tile(0);
+    if (NS * NT > 1) load_tile(1);
   }
 
-  // ------------------------------------------------------------------ consumer warps
   const int  grp    = lane / L;
   const int  gl     = lane % L;
   const bool leader = (gl == 0);
@@ -139,8 +147,8 @@ __global__ void __launch_bounds__((kTW + 1) * 32, 1) mttkrp_tiled_root3(const Ti
 
   // issue side: rounds are enumerated slab-major, then tile-major, at least one (possibly
   // empty) per tile
-  uint32_t it = 0, ioff = 0, ij = 0;
-  auto issue_next = [&]() {
+  uint32_t it = 0, ioff = 0;
+  auto issue_next = [&](uint32_t ij) {      // round ij into stage ij & 1
     if (it >= NS * NT) return;
     uint32_t ws, we;
     part(it % NT, warp * G, (warp + 1) * G, ws, we);
@@ -156,12 +164,11 @@ __global__ void __launch_bounds__((kTW + 1) * 32, 1) mttkrp_tiled_root3(const Ti
         mbar_arrive(bar);
       }
     }
-    ++ij;
     ioff += kTRS;
     if (ws + ioff >= we) { ++it; ioff = 0; }
   };
-  issue_next();
-  issue_next();
+  issue_next(0);
+  issue_next(1);
 
   const double2 zero2 = make_double2(0.0, 0.0);
   double2 acc1 = zero2, acc0 = zero2;      // fiber / slice partial sums
@@ -172,7 +179,7 @@ __global__ void __launch_bounds__((kTW + 1) * 32, 1) mttkrp_tiled_root3(const Ti
     const int    sw   = min(kSlab, a.col_end - sc0);
     const bool   act  = (2 * gl) < sw;
     const int    c2   = act ? 2 * gl : 0;                    // this lane's columns in the slab
-    const char * pbase = reinterpret_cast<const char *>(a.parent + sc0 + c2);
+    const uint32_t poff = static_cast<uint32_t>(sc0 + c2) * 8u;   // this lane's columns of a parent row
     const uint32_t tcol = static_cast<uint32_t>((a.whole ? sc0 : 0) + c2) * 8u;
     double *     abase = accs + c2;
     auto flush = [&](uint32_t n) {                           // the slice closed: into smem
@@ -184,19 +191,19 @@ __global__ void __launch_bounds__((kTW + 1) * 32, 1) mttkrp_tiled_root3(const Ti
 
     for (uint32_t t = 0; t < NT; ++t) {
       const uint32_t gt = s * NT + t;
-      mbar_wait(&tile_full[gt & 1u], (gt >> 1) & 1u);
-      const unsigned char * tile = tiles + (gt & 1u) * a.tile_bytes + tcol;
-      const uint32_t kbase = t * a.tile_rows;
+      // shared address of leaf row 0 (this lane's columns) as if the tile started there
+      const uint32_t tile = smem_u32(tiles) + (gt & 1u) * a.tile_bytes + tcol - t * a.tile_rows * a.tpitch;
       uint32_t ws, we, gs, ge;
       part(t, warp * G, (warp + 1) * G, ws, we);
       part(t, warp * G + grp, warp * G + grp + 1, gs, ge);
       const uint32_t nr = (we > ws) ? (we - ws + kTRS - 1) / kTRS : 1u;
       for (uint32_t i = 0; i < nr; ++i, ++j) {
         mbar_wait(&mybars[j & 1u], (j >> 1) & 1u);
-        SpRec *        buf = myring + (j & 1u) * kTRS;
         const uint32_t rs  = ws + i * kTRS;
         const uint32_t re  = min(we, rs + kTRS);
         const uint32_t lo  = max(gs, rs), hi = min(ge, re);
+        if (i == 0) mbar_wait(&tile_full[gt & 1u], (gt >> 1) & 1u);
+        SpRec *        buf = myring + (j & 1u) * kTRS;
         // the group's last record of this tile closes the slice (sub-range boundary)
         if (leader && hi > lo && hi == ge)
           buf[hi - 1 - rs].aux = (buf[hi - 1 - rs].aux & SPB200_IDX_MASK) | (2u << SPB200_IDX_BITS);
@@ -212,12 +219,13 @@ __global__ void __launch_bounds__((kTW + 1) * 32, 1) mttkrp_tiled_root3(const Ti
               q[u] = *reinterpret_cast<const uint4 *>(&buf[n + u - rs]);
               any |= q[u].w;
             }
+            // leaf rows first: the leaf ids are then dead while the parent rows are in flight
 #pragma unroll
             for (int u = 0; u < kTB; ++u)
-              if (q[u].w >> SPB200_IDX_BITS) r[u] = ld_row_na(pbase, q[u].w & SPB200_IDX_MASK, pitch);
+              b[u] = lds_f64x2(tile + q[u].z * a.tpitch);
 #pragma unroll
             for (int u = 0; u < kTB; ++u)
-              b[u] = *reinterpret_cast<const double2 *>(tile + static_cast<size_t>(q[u].z - kbase) * a.tpitch);
+              if (q[u].w >> SPB200_IDX_BITS) r[u] = ld_row_na(reinterpret_cast<const char *>(a.parent) + poff, q[u].w & SPB200_IDX_MASK, pitch);
             if ((any >> (SPB200_IDX_BITS + 1)) == 0) {
 #pragma unroll
               for (int u = 0; u < kTB; ++u) {
@@ -243,26 +251,34 @@ __global__ void __launch_bounds__((kTW + 1) * 32, 1) mttkrp_tiled_root3(const Ti
             const uint4    q = *reinterpret_cast<const uint4 *>(&buf[n - rs]);
             const double   v = __hiloint2double(static_cast<int>(q.y), static_cast<int>(q.x));
             const uint32_t c = q.w >> SPB200_IDX_BITS;
-            const double2  b = *reinterpret_cast<const double2 *>(tile + static_cast<size_t>(q.z - kbase) * a.tpitch);
+            const double2  b = lds_f64x2(tile + q.z * a.tpitch);
             acc1             = fma2(v, b, acc1);
             if (c) {
-              acc0 = fma2(acc1, ld_row_na(pbase, q.w & SPB200_IDX_MASK, pitch), acc0);
+              acc0 = fma2(acc1, ld_row_na(reinterpret_cast<const char *>(a.parent) + poff, q.w & SPB200_IDX_MASK, pitch), acc0);
               acc1 = zero2;
               if (c >= 2) flush(n);
             }
           }
         }
         __syncwarp();
-        issue_next();        // refill the stage just consumed with round j + 2
+        issue_next(j + 2);   // refill the stage just consumed
       }
+      // this warp is done with tile gt; the last warp to get here loads tile gt + 2 in its place
       __syncwarp();
-      if (lane == 0) mbar_arrive(&tile_empty[gt & 1u]);    // this warp is done with tile gt
+      uint32_t last = 0;
+      if (lane == 0) {
+        __threadfence_block();
+        last = ((atomicAdd(&tile_left[gt & 1u], 1u) + 1u) % kTW == 0) ? 1u : 0u;   // counts on
+        __threadfence_block();
+      }
+      if (__shfl_sync(0xffffffffu, last, 0) && gt + 2 < NS * NT) load_tile(gt + 2);
     }
 
     // the slab is complete: interior rows belong to this range alone and are stored; the
     // first and last row may be shared with the neighbouring ranges and are reduced
-    consumers_sync();
+    __syncthreads();
     const uint32_t pairs = static_cast<uint32_t>(sw) / 2u;
+    const uint32_t nrows = range_rows();
     for (uint32_t i = threadIdx.x; i < nrows * pairs; i += kTW * 32) {
       const uint32_t row = i / pairs, c = 2u * (i % pairs);
       double2 *      src = reinterpret_cast<double2 *>(accs + static_cast<size_t>(row) * kSlab + c);
@@ -276,7 +292,7 @@ __global__ void __launch_bounds__((kTW + 1) * 32, 1) mttkrp_tiled_root3(const Ti
         *reinterpret_cast<double2 *>(dst) = v;
       }
     }
-    consumers_sync();
+    __syncthreads();
   }
 }
 
@@ -314,7 +330,7 @@ int spb200_launch_tiled_root3(const FiberStream & s, int ldm, int col_begin, int
   a.tile_bytes = s.ktile_rows * kSlab * 8u;
   a.tpitch = a.whole ? (uint32_t)ldm * 8u : kSlab * 8u;
   const size_t smem = tiled_smem_bytes(s.ktile_rows, s.acc_rows);
-  const int threads = (kTW + 1) * 32;
+  const int threads = kTW * 32;
   const unsigned grid = s.kranges;
 #define SPB200_TILED_LAUNCH(LL)                                                                   \
   do {                                                                                            \
@@ -324,6 +340,9 @@ int spb200_launch_tiled_root3(const FiberStream & s, int ldm, int col_begin, int
     if (dev_ < 0 || dev_ >= 64 || !set[dev_]) {                                                   \
       SPB200_CUDA_OK(cudaFuncSetAttribute(mttkrp_tiled_root3<LL>,                                 \
                                           cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)); \
+      SPB200_CUDA_OK(cudaFuncSetAttribute(mttkrp_tiled_root3<LL>,                                 \
+                                          cudaFuncAttributePreferredSharedMemoryCarveout,         \
+                                          cudaSharedmemCarveoutMaxShared));                       \
       if (dev_ >= 0 && dev_ < 64) set[dev_] = true;                                               \
     }                                                                                             \
     mttkrp_tiled_root3<LL><<<grid, threads, smem, stream>>>(a);                                   \
