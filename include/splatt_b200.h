@@ -351,7 +351,11 @@ int splatt_b200_mttkrp(
 /* The same for a block of columns only: [col_begin, col_begin + col_count) (col_begin even).
  * MTTKRP is independent per column, so a caller can pipeline column blocks against the
  * PCIe copies of the corresponding factor columns (the drop-in symbols do exactly that
- * when the host buffers are page-locked).  Only those columns of d_out are zeroed/written. */
+ * when the host buffers are page-locked).  Only those columns of d_out are zeroed/written;
+ * an odd col_count also zeroes and writes the one column after the block, so the block must
+ * end at or before the padded rank ncolumns + (ncolumns & 1).  A block with an odd
+ * col_begin, col_begin past the padded rank or col_begin + col_count > ncolumns +
+ * (ncolumns & 1) returns SPLATT_ERROR_BADINPUT and writes nothing. */
 int splatt_b200_mttkrp_columns(
     splatt_b200_tensor const * t,
     int mode,

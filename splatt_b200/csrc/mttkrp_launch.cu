@@ -84,7 +84,9 @@ int spb200_launch_mttkrp(const FiberStream & s, int kind, int outdepth, int ncol
   }
   const int rpad_all = ncolumns + (ncolumns & 1);
   if (col_count <= 0) { col_begin = 0; col_count = rpad_all; }        // whole matrix
-  if ((col_begin & 1) || col_begin < 0 || col_begin + col_count > rpad_all + (col_count & 1) ||
+  // an odd block is widened to the next even column, which must still lie inside rpad_all:
+  // past it the zeroing and the kernel would reach into the next row (or past the buffer)
+  if ((col_begin & 1) || col_begin < 0 || col_count > rpad_all - col_begin ||
       col_begin >= rpad_all) {
     fprintf(stderr, "SPLATT: bad column block [%d, %d) of %d\n", col_begin, col_begin + col_count,
             rpad_all);

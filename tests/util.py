@@ -70,6 +70,7 @@ PARITY_TENSORS = {
     "t4": ((40, 30, 50, 20), 15000),
     "t5": ((12, 15, 10, 20, 9), 8000),
     "t6": ((6, 7, 5, 8, 9, 4), 4000),
+    "t7": ((5, 6, 4, 5, 7, 4, 6), 3500),
     "t8": ((4, 3, 5, 4, 3, 6, 2, 5), 3000),
 }
 
