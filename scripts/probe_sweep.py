@@ -1,8 +1,8 @@
 """Sweep the gather probe (splatt_b200_gather_probe_ex): random whole-row fp64 gathers from an
 L2-resident factor matrix at {1..8} CTAs/SM x {2,4,8,16} rows in flight x {default,
 L1::no_allocate}, an L1 squeeze at the generic root kernel's shape, and the leaf-tiled root
-kernel's shapes (24 and 16 warps/SM, no-allocate, rows in flight x shared memory reserved).  The
-best point is the measured ceiling of the MTTKRP's access pattern.
+kernel's shapes (32, 24 and 16 warps/SM, no-allocate, rows in flight x shared memory reserved).
+The best point is the measured ceiling of the MTTKRP's access pattern.
   python scripts/probe_sweep.py [rows] [rank] [ngathers]
 Prints one JSON line."""
 import ctypes as C
@@ -57,14 +57,16 @@ for na in (0, 1):
             out.append(timed(ctas, rif, na, 0))
 # 2. the MTTKRP kernel's shape (3 CTAs x 8 rows) with less and less L1 left
 l1 = [timed(3, 8, 0, sm) for sm in (0, 8192, 16384, 32768, 49152, 65536, 73728)]
-# 3. the leaf-tiled root kernel's shape: 24 warps/SM (3 x 8), parent rows not allocated in L1,
-#    gathers in flight per lane group x shared memory reserved per CTA (what is left of the
-#    256 KB L1 holds the in-flight lines); and 16 warps/SM (2 x 8), fewer warps with more
-#    registers each
+# 3. the leaf-tiled root kernel's shape: 32 warps/SM (4 x 8; the kernel runs one CTA of 32
+#    warps), parent rows not allocated in L1, gathers in flight per lane group x shared memory
+#    reserved per CTA (what is left of the 256 KB L1 holds the in-flight lines); the earlier
+#    24 warps/SM (3 x 8); and 16 warps/SM (2 x 8), fewer warps with more registers each
 KB = 1024
+tiled32 = [timed(4, rif, 1, sm * KB) for rif in (2, 4, 8) for sm in (0, 32, 48, 55)]
 tiled = [timed(3, rif, 1, sm * KB) for rif in (4, 8, 16) for sm in (0, 16, 32, 48, 64, 72)]
 tiled16 = [timed(2, rif, 1, sm * KB) for rif in (4, 8, 16) for sm in (0, 64, 96, 108)]
 best = max(out, key=lambda r: r["TBps"])
 print(json.dumps({"matrix_rows": rows, "rank": R, "gathers": n, "row_bytes": R * 8,
-                  "best": best, "l1_squeeze_3ctas_8rows": l1, "tiled_shape_24warps": tiled,
+                  "best": best, "l1_squeeze_3ctas_8rows": l1, "tiled_shape_32warps": tiled32,
+                  "tiled_shape_24warps": tiled,
                   "tiled_shape_16warps": tiled16, "sweep": out}))

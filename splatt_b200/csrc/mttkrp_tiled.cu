@@ -25,10 +25,11 @@
 
 namespace spb200 {
 
-constexpr int kTW   = 24;         // warps per CTA, all of them consuming records
-constexpr int kTRS  = 96;         // records per warp per staging round
-constexpr int kTB   = 4;          // records whose gathers are issued together
+constexpr int kTW   = 32;         // warps per CTA, all of them consuming records
+constexpr int kTRS  = 72;         // records per warp per staging round
+constexpr int kTB   = 3;          // records whose gathers are issued together
 constexpr int kSlab = 32;         // columns held in shared memory at a time
+static_assert(kTB <= 4, "a batch's close counts are packed one byte per record");
 
 struct TiledArgs {
   const SpRec *    rec;
@@ -57,11 +58,16 @@ __device__ __forceinline__ double2 lds_f64x2(uint32_t addr) {
   return r;
 }
 
-// Every warp consumes records; there is no separate producer warp.  A 25th warp would cap
-// every thread at 72 registers instead of 80 and the batch loop spilled more (bench.py's
-// headline tensor, H100 80GB HBM3 at 700 W: 0.52 ms per mode with a producer warp, 0.48 ms
-// with this layout).  Leaf tiles are double buffered; the last warp to finish tile gt loads
-// tile gt + 2 into the buffer gt leaves.
+// 32 warps, one CTA per SM, all of them consuming records (no producer warp).  The parent-row
+// gathers are bound by how many warps keep them in flight, not by how deep one warp's batch is
+// (gather probe, DESIGN.md 4.1), and a 1024-thread CTA leaves 64 registers per thread.  The
+// batch loop fits them without spilling: a batch's parent gathers are issued straight from the
+// records' aux words, and the leaf rows are folded into the fiber sums while they are in flight,
+// so only the closing records' fiber products, the parent rows, acc0 / acc1 and the close
+// counts live across the wait.  At 4 records per batch the kernel still spilled (32 B); at 3 it
+// does not.  Per-tile values (segment bounds, the issue side's next round) are re-read rather
+// than held across the batch loop.  Leaf tiles are double buffered; the last warp to finish
+// tile gt loads tile gt + 2 into the buffer gt leaves.
 template <int L>
 __global__ void __launch_bounds__(kTW * 32, 1) mttkrp_tiled_root3(const TiledArgs a) {
   constexpr int G  = 32 / L;
@@ -81,11 +87,11 @@ __global__ void __launch_bounds__(kTW * 32, 1) mttkrp_tiled_root3(const TiledArg
   const uint32_t pitch = static_cast<uint32_t>(a.ldm) * 8u;
   const uint32_t NT    = a.ntiles;
   const uint32_t NS    = static_cast<uint32_t>(a.col_end - a.col0 + kSlab - 1) / kSlab;
-  const uint32_t * so  = a.seg_off + static_cast<size_t>(blockIdx.x) * NT;
-  const uint32_t r_lo  = a.rroot[2 * blockIdx.x];
-  // root rows of this range; re-read where needed rather than held across the main loop
+  // the range's first root row, its row count and its segment offsets are re-read where needed
+  // rather than held in registers across the main loop
+  auto range_lo   = [&]() { return __ldg(&a.rroot[2 * blockIdx.x]); };
   auto range_rows = [&]() {
-    const uint32_t r_hi = __ldg(&a.rroot[2 * blockIdx.x + 1]);
+    const uint32_t r_lo = range_lo(), r_hi = __ldg(&a.rroot[2 * blockIdx.x + 1]);
     return (r_hi >= r_lo) ? r_hi - r_lo + 1 : 0u;
   };
 
@@ -140,32 +146,35 @@ __global__ void __launch_bounds__(kTW * 32, 1) mttkrp_tiled_root3(const TiledArg
 
   // part of segment t that belongs to lane-group gi / to this warp
   auto part = [&](uint32_t t, uint32_t g0, uint32_t g1, uint32_t & lo, uint32_t & hi) {
-    const uint32_t s0 = so[t], len = so[t + 1] - s0;
+    const uint32_t * so = a.seg_off + blockIdx.x * NT + t;
+    const uint32_t s0 = __ldg(so), len = __ldg(so + 1) - s0;
     lo = s0 + static_cast<uint32_t>(static_cast<unsigned long long>(g0) * len / NG);
     hi = s0 + static_cast<uint32_t>(static_cast<unsigned long long>(g1) * len / NG);
   };
 
-  // issue side: rounds are enumerated slab-major, then tile-major, at least one (possibly
-  // empty) per tile
-  uint32_t it = 0, ioff = 0;
+  // issue side, run by lane 0: rounds are enumerated slab-major, then tile-major, at least one
+  // (possibly empty) per tile; the next round to issue (tile, offset) is kept in shared memory
+  uint32_t * inext = reinterpret_cast<uint32_t *>(rec_full + 2 * kTW) + 2 * warp;
+  if (lane == 0) { inext[0] = 0; inext[1] = 0; }
   auto issue_next = [&](uint32_t ij) {      // round ij into stage ij & 1
+    if (lane != 0) return;
+    uint32_t it = inext[0], ioff = inext[1];
     if (it >= NS * NT) return;
     uint32_t ws, we;
     part(it % NT, warp * G, (warp + 1) * G, ws, we);
     const uint32_t rs  = ws + ioff;
     const uint32_t cnt = (rs < we) ? min(static_cast<uint32_t>(kTRS), we - rs) : 0u;
-    if (lane == 0) {
-      uint64_t * bar = &mybars[ij & 1u];
-      if (cnt) {
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        mbar_arrive_expect_tx(bar, cnt * 16u);
-        tma_bulk_g2s(myring + (ij & 1u) * kTRS, a.rec + rs, cnt * 16u, bar);
-      } else {
-        mbar_arrive(bar);
-      }
+    uint64_t * bar = &mybars[ij & 1u];
+    if (cnt) {
+      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+      mbar_arrive_expect_tx(bar, cnt * 16u);
+      tma_bulk_g2s(myring + (ij & 1u) * kTRS, a.rec + rs, cnt * 16u, bar);
+    } else {
+      mbar_arrive(bar);
     }
     ioff += kTRS;
     if (ws + ioff >= we) { ++it; ioff = 0; }
+    inext[0] = it; inext[1] = ioff;
   };
   issue_next(0);
   issue_next(1);
@@ -174,111 +183,123 @@ __global__ void __launch_bounds__(kTW * 32, 1) mttkrp_tiled_root3(const TiledArg
   double2 acc1 = zero2, acc0 = zero2;      // fiber / slice partial sums
   uint32_t j = 0;                          // rounds consumed
 
-  for (uint32_t s = 0; s < NS; ++s) {
-    const int    sc0  = a.col0 + static_cast<int>(s) * kSlab;
-    const int    sw   = min(kSlab, a.col_end - sc0);
-    const bool   act  = (2 * gl) < sw;
-    const int    c2   = act ? 2 * gl : 0;                    // this lane's columns in the slab
+  // tiles gt in order, slab-major: slab gt / NT, leaf tile gt % NT
+  for (uint32_t gt = 0; gt < NS * NT; ++gt) {
+    const uint32_t s    = gt / NT, t = gt - s * NT;
+    const int      sc0  = a.col0 + static_cast<int>(s) * kSlab;
+    const int      sw   = min(kSlab, a.col_end - sc0);
+    const bool     act  = (2 * gl) < sw;
+    const int      c2   = act ? 2 * gl : 0;                    // this lane's columns in the slab
     const uint32_t poff = static_cast<uint32_t>(sc0 + c2) * 8u;   // this lane's columns of a parent row
     const uint32_t tcol = static_cast<uint32_t>((a.whole ? sc0 : 0) + c2) * 8u;
-    double *     abase = accs + c2;
+    double *       abase = accs + c2;
+    // the lanes of this lane group that run the batch loop (they take the same trips)
+    const uint32_t gmask = ((1u << min(L, (sw + 1) / 2)) - 1u) << (grp * L);
     auto flush = [&](uint32_t n) {                           // the slice closed: into smem
-      double * p = abase + static_cast<size_t>(__ldg(&a.rootid[n]) - r_lo) * kSlab;
+      double * p = abase + static_cast<size_t>(__ldg(&a.rootid[n]) - range_lo()) * kSlab;
       atomicAdd(p, acc0.x);
       atomicAdd(p + 1, acc0.y);
       acc0 = zero2;
     };
-
-    for (uint32_t t = 0; t < NT; ++t) {
-      const uint32_t gt = s * NT + t;
-      // shared address of leaf row 0 (this lane's columns) as if the tile started there
-      const uint32_t tile = smem_u32(tiles) + (gt & 1u) * a.tile_bytes + tcol - t * a.tile_rows * a.tpitch;
+    // shared address of leaf row 0 (this lane's columns) as if the tile started there
+    const uint32_t tile = smem_u32(tiles) + (gt & 1u) * a.tile_bytes + tcol - t * a.tile_rows * a.tpitch;
+    // one or more rounds per tile (one, for a tile no larger than the policy picks); the
+    // segment bounds are re-read every round rather than held across the batch loop
+    for (uint32_t i = 0, more = 1; more; ++i, ++j) {
       uint32_t ws, we, gs, ge;
       part(t, warp * G, (warp + 1) * G, ws, we);
       part(t, warp * G + grp, warp * G + grp + 1, gs, ge);
-      const uint32_t nr = (we > ws) ? (we - ws + kTRS - 1) / kTRS : 1u;
-      for (uint32_t i = 0; i < nr; ++i, ++j) {
-        mbar_wait(&mybars[j & 1u], (j >> 1) & 1u);
-        const uint32_t rs  = ws + i * kTRS;
-        const uint32_t re  = min(we, rs + kTRS);
-        const uint32_t lo  = max(gs, rs), hi = min(ge, re);
-        if (i == 0) mbar_wait(&tile_full[gt & 1u], (gt >> 1) & 1u);
-        SpRec *        buf = myring + (j & 1u) * kTRS;
-        // the group's last record of this tile closes the slice (sub-range boundary)
-        if (leader && hi > lo && hi == ge)
-          buf[hi - 1 - rs].aux = (buf[hi - 1 - rs].aux & SPB200_IDX_MASK) | (2u << SPB200_IDX_BITS);
-        __syncwarp();
-        if (act && hi > lo) {
-          uint32_t n = lo;
-          for (; n + kTB <= hi; n += kTB) {
-            uint4   q[kTB];
-            double2 b[kTB], r[kTB];
-            uint32_t any = 0;
+      mbar_wait(&mybars[j & 1u], (j >> 1) & 1u);
+      const uint32_t rs  = ws + i * kTRS;
+      const uint32_t re  = min(we, rs + kTRS);
+      const uint32_t lo  = max(gs, rs), hi = min(ge, re);
+      more = (re < we) ? 1u : 0u;
+      if (i == 0) mbar_wait(&tile_full[gt & 1u], (gt >> 1) & 1u);
+      SpRec *        buf = myring + (j & 1u) * kTRS;
+      // the group's last record of this tile closes the slice (sub-range boundary)
+      if (leader && hi > lo && hi == ge)
+        buf[hi - 1 - rs].aux = (buf[hi - 1 - rs].aux & SPB200_IDX_MASK) | (2u << SPB200_IDX_BITS);
+      __syncwarp();
+      if (act && hi > lo) {
+        uint32_t n = lo;
+        for (; n + kTB <= hi; n += kTB) {
+          const SpRec * bq = buf + (n - rs);
+          // parent gathers first, from the records' aux words; the close counts are kept one
+          // byte per record
+          double2  r[kTB];
+          uint32_t cc = 0;
+#pragma unroll
+          for (int u = 0; u < kTB; ++u) {
+            const uint32_t w = bq[u].aux;
+            cc |= (w >> SPB200_IDX_BITS) << (8 * u);
+            if (w >> SPB200_IDX_BITS) r[u] = ld_row_na(reinterpret_cast<const char *>(a.parent) + poff, w & SPB200_IDX_MASK, pitch);
+          }
+          // keeps the gathers ahead of the leaf fold: without it ptxas sinks them below the
+          // first records' leaf reads to save registers (0.46 against 0.45 ms per mode)
+          __syncwarp(gmask);
+          // while they are in flight, the leaf rows fold into the fiber sums; a closing
+          // record's fiber product waits in p[u] for its parent row (the last record's stays
+          // in acc1, and p[kTB - 1] is never set)
+          double2 p[kTB];
+#pragma unroll
+          for (int u = 0; u < kTB; ++u) {
+            const uint4  q = *reinterpret_cast<const uint4 *>(&bq[u]);
+            const double v = __hiloint2double(static_cast<int>(q.y), static_cast<int>(q.x));
+            acc1           = fma2(v, lds_f64x2(tile + q.z * a.tpitch), acc1);
+            if (u + 1 < kTB && ((cc >> (8 * u)) & 0xffu)) { p[u] = acc1; acc1 = zero2; }
+          }
+          auto close = [&](int u) {
+            acc0 = fma2(u + 1 < kTB ? p[u] : acc1, r[u], acc0);
+            if (u + 1 == kTB) acc1 = zero2;
+          };
+          if ((cc & 0xfefefefeu) == 0) {             // no slice ends in the batch
+#pragma unroll
+            for (int u = 0; u < kTB; ++u)
+              if ((cc >> (8 * u)) & 0xffu) close(u);
+          } else {
 #pragma unroll
             for (int u = 0; u < kTB; ++u) {
-              q[u] = *reinterpret_cast<const uint4 *>(&buf[n + u - rs]);
-              any |= q[u].w;
-            }
-            // leaf rows first: the leaf ids are then dead while the parent rows are in flight
-#pragma unroll
-            for (int u = 0; u < kTB; ++u)
-              b[u] = lds_f64x2(tile + q[u].z * a.tpitch);
-#pragma unroll
-            for (int u = 0; u < kTB; ++u)
-              if (q[u].w >> SPB200_IDX_BITS) r[u] = ld_row_na(reinterpret_cast<const char *>(a.parent) + poff, q[u].w & SPB200_IDX_MASK, pitch);
-            if ((any >> (SPB200_IDX_BITS + 1)) == 0) {
-#pragma unroll
-              for (int u = 0; u < kTB; ++u) {
-                const double v = __hiloint2double(static_cast<int>(q[u].y), static_cast<int>(q[u].x));
-                acc1           = fma2(v, b[u], acc1);
-                if (q[u].w >> SPB200_IDX_BITS) { acc0 = fma2(acc1, r[u], acc0); acc1 = zero2; }
+              const uint32_t c = (cc >> (8 * u)) & 0xffu;
+              if (c) {
+                close(u);
+                if (c >= 2) flush(n + u);
               }
-            } else {
-#pragma unroll
-              for (int u = 0; u < kTB; ++u) {
-                const double   v = __hiloint2double(static_cast<int>(q[u].y), static_cast<int>(q[u].x));
-                const uint32_t c = q[u].w >> SPB200_IDX_BITS;
-                acc1             = fma2(v, b[u], acc1);
-                if (c) {
-                  acc0 = fma2(acc1, r[u], acc0);
-                  acc1 = zero2;
-                  if (c >= 2) flush(n + u);
-                }
-              }
-            }
-          }
-          for (; n < hi; ++n) {
-            const uint4    q = *reinterpret_cast<const uint4 *>(&buf[n - rs]);
-            const double   v = __hiloint2double(static_cast<int>(q.y), static_cast<int>(q.x));
-            const uint32_t c = q.w >> SPB200_IDX_BITS;
-            const double2  b = lds_f64x2(tile + q.z * a.tpitch);
-            acc1             = fma2(v, b, acc1);
-            if (c) {
-              acc0 = fma2(acc1, ld_row_na(reinterpret_cast<const char *>(a.parent) + poff, q.w & SPB200_IDX_MASK, pitch), acc0);
-              acc1 = zero2;
-              if (c >= 2) flush(n);
             }
           }
         }
-        __syncwarp();
-        issue_next(j + 2);   // refill the stage just consumed
+#pragma unroll 1
+        for (; n < hi; ++n) {
+          const uint4    q = *reinterpret_cast<const uint4 *>(&buf[n - rs]);
+          const double   v = __hiloint2double(static_cast<int>(q.y), static_cast<int>(q.x));
+          const uint32_t c = q.w >> SPB200_IDX_BITS;
+          const double2  b = lds_f64x2(tile + q.z * a.tpitch);
+          acc1             = fma2(v, b, acc1);
+          if (c) {
+            acc0 = fma2(acc1, ld_row_na(reinterpret_cast<const char *>(a.parent) + poff, q.w & SPB200_IDX_MASK, pitch), acc0);
+            acc1 = zero2;
+            if (c >= 2) flush(n);
+          }
+        }
       }
-      // this warp is done with tile gt; the last warp to get here loads tile gt + 2 in its place
       __syncwarp();
-      uint32_t last = 0;
-      if (lane == 0) {
-        __threadfence_block();
-        last = ((atomicAdd(&tile_left[gt & 1u], 1u) + 1u) % kTW == 0) ? 1u : 0u;   // counts on
-        __threadfence_block();
-      }
-      if (__shfl_sync(0xffffffffu, last, 0) && gt + 2 < NS * NT) load_tile(gt + 2);
+      issue_next(j + 2);   // refill the stage just consumed
     }
+    // this warp is done with tile gt; the last warp to get here loads tile gt + 2 in its place
+    __syncwarp();
+    uint32_t last = 0;
+    if (lane == 0) {
+      __threadfence_block();
+      last = ((atomicAdd(&tile_left[gt & 1u], 1u) + 1u) % kTW == 0) ? 1u : 0u;   // counts on
+      __threadfence_block();
+    }
+    if (__shfl_sync(0xffffffffu, last, 0) && gt + 2 < NS * NT) load_tile(gt + 2);
 
+    if (t + 1 < NT) continue;
     // the slab is complete: interior rows belong to this range alone and are stored; the
     // first and last row may be shared with the neighbouring ranges and are reduced
     __syncthreads();
     const uint32_t pairs = static_cast<uint32_t>(sw) / 2u;
-    const uint32_t nrows = range_rows();
+    const uint32_t nrows = range_rows(), r_lo = range_lo();
     for (uint32_t i = threadIdx.x; i < nrows * pairs; i += kTW * 32) {
       const uint32_t row = i / pairs, c = 2u * (i % pairs);
       double2 *      src = reinterpret_cast<double2 *>(accs + static_cast<size_t>(row) * kSlab + c);
@@ -302,7 +323,7 @@ __global__ void __launch_bounds__(kTW * 32, 1) mttkrp_tiled_root3(const TiledArg
 static size_t tiled_smem_bytes(uint32_t tile_rows, uint32_t acc_rows) {
   using namespace spb200;
   return (2 * (size_t)tile_rows + acc_rows) * kSlab * 8 + sizeof(SpRec) * kTW * 2 * kTRS +
-         sizeof(uint64_t) * (4 + 2 * kTW) + 128;
+         sizeof(uint64_t) * (4 + 3 * kTW) + 128;
 }
 
 uint32_t spb200_tiled_rows_for(uint32_t acc_rows) {
