@@ -348,6 +348,24 @@ int splatt_b200_mttkrp(
     double * d_out,
     void * stream);
 
+/* Single precision: the same product with float factors and a float output, for callers whose
+ * factors are fp32 (e.g. PyTorch defaults).  Every nonzero's value is rounded to fp32 once
+ * and products and sums are formed in fp32; the tensor is the one splatt_b200_mttkrp uses
+ * (no rebuild).  Contract as splatt_b200_mttkrp -- d_out zeroed, then accumulated into;
+ * sharded tensors give partial sums; no host synchronisation; d_mats[mode] ignored -- except
+ * the alignment rules: ldm % 4 == 0, ldm >= (ncolumns + 3) & ~3, and every base pointer
+ * 16-byte aligned.  A violation returns SPLATT_ERROR_BADINPUT and writes nothing.
+ * Columns [(ncolumns + 3) & ~3, ldm) of d_out are left zero; [ncolumns, (ncolumns + 3) & ~3)
+ * are unspecified.  The f32 reductions flush subnormal sums to zero. */
+int splatt_b200_mttkrp_f32(
+    splatt_b200_tensor const * t,
+    int mode,
+    int ncolumns,
+    int ldm,
+    float const * const * d_mats,
+    float * d_out,
+    void * stream);
+
 /* The same for a block of columns only: [col_begin, col_begin + col_count) (col_begin even).
  * MTTKRP is independent per column, so a caller can pipeline column blocks against the
  * PCIe copies of the corresponding factor columns (the drop-in symbols do exactly that

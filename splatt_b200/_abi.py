@@ -29,6 +29,7 @@ idx_t = C.c_uint64
 val_t = C.c_double
 idx_p = C.POINTER(idx_t)
 val_p = C.POINTER(val_t)
+f32_p = C.POINTER(C.c_float)
 
 
 class CsfSparsity(C.Structure):
@@ -95,7 +96,7 @@ EXPORTS = [
     "splatt_cpd_als", "splatt_free_kruskal", "splatt_default_opts", "splatt_free_opts",
     "splatt_b200_tensor_from_csf", "splatt_b200_tensor_from_coo", "splatt_b200_tensor_free",
     "splatt_b200_tensor_info", "splatt_b200_mode_info", "splatt_b200_csf_alloc",
-    "splatt_b200_csf_free", "splatt_b200_mttkrp", "splatt_b200_launch_count",
+    "splatt_b200_csf_free", "splatt_b200_mttkrp", "splatt_b200_mttkrp_f32", "splatt_b200_launch_count",
     "splatt_b200_version", "splatt_b200_level_orders", "splatt_b200_cta_tiling", "splatt_b200_shard_range", "splatt_b200_mttkrp_multicast", "splatt_b200_gather_probe", "splatt_b200_gather_probe_ex", "splatt_b200_mttkrp_columns",
     "splatt_b200_als_tail_create", "splatt_b200_als_tail_free", "splatt_b200_als_tail_gram",
     "splatt_b200_als_tail_update", "splatt_b200_als_tail_fit", "splatt_b200_csf_to_coo",
@@ -164,6 +165,9 @@ def load() -> C.CDLL:
     lib.splatt_b200_mttkrp.restype = C.c_int
     lib.splatt_b200_mttkrp.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, vpp, val_p,
                                        C.c_void_p]
+    lib.splatt_b200_mttkrp_f32.restype = C.c_int
+    lib.splatt_b200_mttkrp_f32.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int,
+                                           C.POINTER(f32_p), f32_p, C.c_void_p]
     lib.splatt_b200_mttkrp_multicast.restype = C.c_int
     lib.splatt_b200_mttkrp_multicast.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, vpp, val_p,
                                                  C.c_void_p]

@@ -235,7 +235,8 @@ class Tensor:
                  layout: int = A.LAYOUT_ALLROOT, device: int = -1, shard_rank: int = 0,
                  shard_count: int = 1, verbosity: int = 0, ncolumns_hint: int = 0,
                  ktile: int = 0) -> "Tensor":
-        """ind/vals: numpy (host) arrays, or torch CUDA tensors (int32/uint32 + float64).
+        """ind/vals: numpy (host) arrays, or torch CUDA tensors (int32/uint32 + float64 or
+        float32; float32 values are widened exactly to float64).
         ncolumns_hint: the rank the tensor will be multiplied at (enables leaf tiling)."""
         lib = A.load()
         on_device = 0
@@ -252,6 +253,10 @@ class Tensor:
             nm = len(dims_a)
             nnz = int(vals.numel())
             keep = [i.contiguous() for i in ind]
+            if vals.dtype == torch.float32:
+                vals = vals.to(torch.float64)            # exact
+            elif vals.dtype != torch.float64:
+                raise ValueError(f"device values must be float64 or float32, not {vals.dtype}")
             v = vals.contiguous()
             ip = (C.POINTER(C.c_uint32) * nm)(
                 *[C.cast(C.c_void_p(i.data_ptr()), C.POINTER(C.c_uint32)) for i in keep])
@@ -290,27 +295,37 @@ class Tensor:
                 "alg_bytes": int(ab.value)}
 
     def mttkrp(self, mode: int, mats, out, ncolumns: Optional[int] = None, stream=None):
-        """Enqueue one MTTKRP.  mats[m], out: torch CUDA float64, row-major, same even
-        leading dimension (>= ncolumns).  No host sync."""
+        """Enqueue one MTTKRP.  mats[m], out: torch CUDA tensors of one dtype, row-major, same
+        leading dimension (>= ncolumns).  float64: the leading dimension is even.  float32
+        (splatt_b200_mttkrp_f32: fp32 arithmetic): it is a multiple of 4.  No host sync."""
         import torch
+        if out.dtype == torch.float64:
+            ptr_t, sym, align = A.val_p, "splatt_b200_mttkrp", "even"
+        elif out.dtype == torch.float32:
+            ptr_t, sym, align = A.f32_p, "splatt_b200_mttkrp_f32", "a multiple of 4"
+        else:
+            raise ValueError(f"MTTKRP output must be float64 or float32, not {out.dtype}")
         ldm = out.stride(0)
+        if out.dtype == torch.float32 and ldm % 4:
+            raise ValueError(f"float32 MTTKRP needs a leading dimension (stride(0)) that is a "
+                             f"multiple of 4, got {ldm}")
         R = out.shape[1] if ncolumns is None else ncolumns
-        ptrs = (A.val_p * self.nmodes)()
+        ptrs = (ptr_t * self.nmodes)()
         for m in range(self.nmodes):
             if m == mode or mats[m] is None:
-                ptrs[m] = A.val_p()
+                ptrs[m] = ptr_t()
                 continue
             t = mats[m]
-            if not (t.is_cuda and t.dtype == torch.float64 and t.stride(1) == 1 and
-                    t.stride(0) == ldm):
-                raise ValueError("factor matrices must be CUDA float64 row-major with the "
-                                 "output's leading dimension")
-            ptrs[m] = C.cast(C.c_void_p(t.data_ptr()), A.val_p)
+            if t.dtype != out.dtype:
+                raise ValueError(f"factor matrix {m} is {t.dtype} but the output is {out.dtype}")
+            if not (t.is_cuda and t.stride(1) == 1 and t.stride(0) == ldm):
+                raise ValueError(f"factor matrices must be CUDA {out.dtype} row-major with the "
+                                 f"output's leading dimension ({align})")
+            ptrs[m] = C.cast(C.c_void_p(t.data_ptr()), ptr_t)
         s = torch.cuda.current_stream().cuda_stream if stream is None else stream
-        rc = self.lib.splatt_b200_mttkrp(self.h, mode, R, ldm, ptrs,
-                                         C.cast(C.c_void_p(out.data_ptr()), A.val_p),
-                                         C.c_void_p(s))
-        _check(rc, "splatt_b200_mttkrp")
+        rc = getattr(self.lib, sym)(self.h, mode, R, ldm, ptrs,
+                                    C.cast(C.c_void_p(out.data_ptr()), ptr_t), C.c_void_p(s))
+        _check(rc, sym)
         return out
 
     def shard(self, rank: int, count: int, device: int = -1) -> "Tensor":

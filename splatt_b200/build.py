@@ -30,6 +30,8 @@ def _units():
     units = []
     for n in range(2, 9):
         units.append((f"mttkrp_inst_n{n}", CSRC / "mttkrp_inst.cu", [f"-DSPB200_INST_N={n}"]))
+        units.append((f"mttkrp_inst_f32_n{n}", CSRC / "mttkrp_inst.cu",
+                      [f"-DSPB200_INST_N={n}", "-DSPB200_INST_F32"]))
     for name in ("mttkrp_launch", "mttkrp_tiled", "stream_build", "engine", "dropin", "cpd", "multi"):
         units.append((name, CSRC / f"{name}.cu", []))
     return units

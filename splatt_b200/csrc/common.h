@@ -107,12 +107,12 @@ struct MttkrpArgs {
   const uint32_t * up[SPB200_MAXN - 2];
   const uint32_t * desc;
   const uint32_t * anc;                 // N >= 4 root kernels: level-(N-3) index per record
-  const double *   mats[SPB200_MAXN];   // by LEVEL: factor of mode perm[l]
-  double *         out;
+  const void *     mats[SPB200_MAXN];   // by LEVEL: factor of mode perm[l] (the kernel's value type)
+  void *           out;
   unsigned long long nrec;
   unsigned int     nchunks;
-  int              ldm;       // leading dimension of every matrix (doubles, even)
-  int              ncols;     // active columns in this launch (even, <= 2*L)
+  int              ldm;       // leading dimension of every matrix (elements; 16 B multiple)
+  int              ncols;     // active columns in this launch (16 B multiple, <= L * 16 B)
   int              col0;      // first column of this launch
   int              outdepth;  // level of the output mode
   int              ktiled;    // stream is leaf-tile ordered: keep non-leaf gathers out of L1
@@ -181,6 +181,11 @@ int spb200_launch_mttkrp(const FiberStream & s, int kind, int outdepth,
                          const double * const * d_mats_by_mode, double * d_out,
                          uint64_t out_rows, cudaStream_t stream, bool multicast_out = false,
                          int col_begin = 0, int col_count = 0, const GroupSync * sync = nullptr);
+// The same in fp32 (factors and output float, records rounded to fp32, fp32 arithmetic): whole
+// matrices only, never multicast, never the CTA-tiled kernel.  ldm % 4 == 0.
+int spb200_launch_mttkrp_f32(const FiberStream & s, int kind, int outdepth, int ncolumns, int ldm,
+                             const float * const * d_mats_by_mode, float * d_out,
+                             uint64_t out_rows, cudaStream_t stream);
 extern unsigned long long g_spb200_launches;
 extern unsigned long long g_spb200_builds;     // fiber streams built (sort + scans) so far
 inline void spb200_count_launches(unsigned n) { __atomic_fetch_add(&g_spb200_launches, n, __ATOMIC_RELAXED); }

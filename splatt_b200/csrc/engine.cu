@@ -509,6 +509,19 @@ int splatt_b200_mttkrp(splatt_b200_tensor const * t, int mode, int ncolumns, int
                               d_out, t->dims[mode], static_cast<cudaStream_t>(stream));
 }
 
+int splatt_b200_mttkrp_f32(splatt_b200_tensor const * t, int mode, int ncolumns, int ldm,
+                           float const * const * d_mats, float * d_out, void * stream) {
+  if (!t || !d_mats || !d_out || mode < 0 || mode >= t->nmodes) {
+    fprintf(stderr, "SPLATT: splatt_b200_mttkrp_f32: bad arguments\n");
+    return SPLATT_ERROR_BADINPUT;
+  }
+  const ModePlan & p = t->plan[mode];
+  DeviceGuard g(t->device);
+  if (!g.ok) return SPLATT_ERROR_BADINPUT;
+  return spb200_launch_mttkrp_f32(t->streams[p.stream], p.kind, p.outdepth, ncolumns, ldm, d_mats,
+                                  d_out, t->dims[mode], static_cast<cudaStream_t>(stream));
+}
+
 int splatt_b200_mttkrp_columns(splatt_b200_tensor const * t, int mode, int ncolumns, int ldm,
                                double const * const * d_mats, double * d_out, int col_begin,
                                int col_count, void * stream) {

@@ -10,10 +10,10 @@
 //
 // Execution model
 // ---------------
-//  * A "group" of L lanes owns one record at a time; each lane carries two
-//    adjacent fp64 columns, so a factor row is fetched with one 128-bit load
-//    per lane (L = 16 covers R <= 32, L = 32 covers R <= 64, ...).  A warp
-//    holds 32/L independent groups.
+//  * A "group" of L lanes owns one record at a time; each lane carries one 128-bit
+//    vector of adjacent columns (LaneVec: two fp64 or four fp32 columns), so a factor
+//    row is fetched with one 128-bit load per lane (fp64: L = 16 covers R <= 32,
+//    L = 32 covers R <= 64; fp32: twice that).  A warp holds 32/L independent groups.
 //  * Every group walks ONE contiguous range of the stream (nnz-balanced:
 //    ranges are equal record counts, not equal slice counts, so skewed slices
 //    cannot unbalance the machine).  The tree is traversed by counting close
@@ -94,19 +94,36 @@ __device__ __forceinline__ void tma_bulk_g2s(void * dst, const void * src, uint3
       : "memory");
 }
 
-// Row addressing: `base` already points at this lane's column pair; the row offset
+// One lane's share of a factor row: 16 bytes, i.e. W columns of the value type T.
+template <typename T> struct LaneVec;
+template <> struct LaneVec<double> { using type = double2; static constexpr int W = 2; };
+template <> struct LaneVec<float>  { using type = float4;  static constexpr int W = 4; };
+
+// Row addressing: `base` already points at this lane's columns; the row offset
 // is one 32x32->64 multiply-add (IMAD.WIDE.U32) of the index with the row pitch.
-__device__ __forceinline__ double2 ld_row(const char * __restrict__ base, uint32_t idx,
-                                          uint32_t pitch) {
-  return __ldg(reinterpret_cast<const double2 *>(base + static_cast<uint64_t>(idx) * pitch));
+template <typename V = double2>
+__device__ __forceinline__ V ld_row(const char * __restrict__ base, uint32_t idx, uint32_t pitch) {
+  return __ldg(reinterpret_cast<const V *>(base + static_cast<uint64_t>(idx) * pitch));
 }
 // Same gather, but the line is not allocated in L1 (parent rows of a leaf-tiled stream
 // are touched once per SM: keeping them out leaves L1 to the leaf tile).
-__device__ __forceinline__ double2 ld_row_na(const char * __restrict__ base, uint32_t idx,
-                                             uint32_t pitch) {
+template <typename V = double2>
+__device__ __forceinline__ V ld_row_na(const char * __restrict__ base, uint32_t idx, uint32_t pitch);
+template <>
+__device__ __forceinline__ double2 ld_row_na<double2>(const char * __restrict__ base, uint32_t idx,
+                                                      uint32_t pitch) {
   double2 r;
   asm("ld.global.nc.L1::no_allocate.v2.f64 {%0, %1}, [%2];"
                : "=d"(r.x), "=d"(r.y)
+               : "l"(base + static_cast<uint64_t>(idx) * pitch));
+  return r;
+}
+template <>
+__device__ __forceinline__ float4 ld_row_na<float4>(const char * __restrict__ base, uint32_t idx,
+                                                    uint32_t pitch) {
+  float4 r;
+  asm("ld.global.nc.L1::no_allocate.v4.f32 {%0, %1, %2, %3}, [%4];"
+               : "=f"(r.x), "=f"(r.y), "=f"(r.z), "=f"(r.w)
                : "l"(base + static_cast<uint64_t>(idx) * pitch));
   return r;
 }
@@ -115,6 +132,14 @@ __device__ __forceinline__ void red_row(char * __restrict__ base, uint32_t idx, 
   double * p = reinterpret_cast<double *>(base + static_cast<uint64_t>(idx) * pitch);
   atomicAdd(p, x.x);      // result unused -> RED.E.ADD.F64
   atomicAdd(p + 1, x.y);
+}
+// One vector reduction for the four columns (REDG.E.ADD.F32x4).  Like every f32 global
+// reduction it flushes subnormal operands and results to (sign-preserving) zero.
+__device__ __forceinline__ void red_row(char * __restrict__ base, uint32_t idx, uint32_t pitch,
+                                        float4 x) {
+  float * p = reinterpret_cast<float *>(base + static_cast<uint64_t>(idx) * pitch);
+  asm volatile("red.relaxed.gpu.global.add.v4.f32 [%0], {%1, %2, %3, %4};"
+               ::"l"(p), "f"(x.x), "f"(x.y), "f"(x.z), "f"(x.w) : "memory");
 }
 // The same reduction through an NVLink MULTICAST address: one instruction adds the value
 // into the row of every GPU of the group (NVSwitch fans it out).  Used by the fused
@@ -148,43 +173,69 @@ __device__ __forceinline__ void st_row_mc(char * __restrict__ base, uint32_t idx
   double * p = reinterpret_cast<double *>(base + static_cast<uint64_t>(idx) * pitch);
   asm volatile("st.relaxed.sys.global.v2.f64 [%0], {%1, %2};" ::"l"(p), "d"(x.x), "d"(x.y) : "memory");
 }
-__device__ __forceinline__ double2 fma2(double s, double2 a, double2 c) {
+__device__ __forceinline__ double2 vfma(double s, double2 a, double2 c) {
   return make_double2(fma(s, a.x, c.x), fma(s, a.y, c.y));
 }
-__device__ __forceinline__ double2 fma2(double2 a, double2 b, double2 c) {
+__device__ __forceinline__ double2 vfma(double2 a, double2 b, double2 c) {
   return make_double2(fma(a.x, b.x, c.x), fma(a.y, b.y, c.y));
 }
-__device__ __forceinline__ double2 mul2(double2 a, double2 b) {
+__device__ __forceinline__ double2 vmul(double2 a, double2 b) {
   return make_double2(a.x * b.x, a.y * b.y);
 }
+__device__ __forceinline__ double2 vmul(double s, double2 a) {
+  return make_double2(s * a.x, s * a.y);
+}
+__device__ __forceinline__ float4 vfma(float s, float4 a, float4 c) {
+  return make_float4(fmaf(s, a.x, c.x), fmaf(s, a.y, c.y), fmaf(s, a.z, c.z), fmaf(s, a.w, c.w));
+}
+__device__ __forceinline__ float4 vfma(float4 a, float4 b, float4 c) {
+  return make_float4(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y), fmaf(a.z, b.z, c.z),
+                     fmaf(a.w, b.w, c.w));
+}
+__device__ __forceinline__ float4 vmul(float4 a, float4 b) {
+  return make_float4(a.x * b.x, a.y * b.y, a.z * b.z, a.w * b.w);
+}
+__device__ __forceinline__ float4 vmul(float s, float4 a) {
+  return make_float4(s * a.x, s * a.y, s * a.z, s * a.w);
+}
+template <typename V> __device__ __forceinline__ V vzero();
+template <> __device__ __forceinline__ double2 vzero<double2>() { return make_double2(0.0, 0.0); }
+template <> __device__ __forceinline__ float4 vzero<float4>() { return make_float4(0.f, 0.f, 0.f, 0.f); }
+// The record's value in the kernel's value type (fp32: rounded once, to nearest).
+template <typename T> __device__ __forceinline__ T rec_val(const uint4 q) {
+  return static_cast<T>(__hiloint2double(static_cast<int>(q.y), static_cast<int>(q.x)));
+}
+
+// Minimum CTAs per SM a stream kernel is compiled for unless a variant names its own.
+__host__ __device__ constexpr int default_minb(int N, int BATCH) { return (BATCH >= 8 || N >= 4) ? 2 : 3; }
 
 // One record of the root traversal (levels above the leaf fold upwards; the
 // root row leaves the SM with a RED).  `b`/`r` are the gathered leaf / parent
 // rows; for N >= 4 `r2` is the gathered level-(N-3) row (valid when c >= 2).
-template <int N, bool MC>
-__device__ __forceinline__ void root_record(const MttkrpArgs & a, const uint4 q, const double2 b,
-                                            const double2 r, const double2 r2,
-                                            double2 (&acc)[N - 1], uint32_t (&pos)[(N > 2) ? N - 2 : 1],
+template <typename Val, int N, bool MC, typename V = typename LaneVec<Val>::type>
+__device__ __forceinline__ void root_record(const MttkrpArgs & a, const uint4 q, const V b,
+                                            const V r, const V r2,
+                                            V (&acc)[N - 1], uint32_t (&pos)[(N > 2) ? N - 2 : 1],
                                             const char * const (&mbase)[N], char * obase,
                                             uint32_t pitch, bool & seen_root, const bool last) {
-  const double2  zero2 = make_double2(0.0, 0.0);
-  const double   v     = __hiloint2double(static_cast<int>(q.y), static_cast<int>(q.x));
+  const V        zero2 = vzero<V>();
+  const Val      v     = rec_val<Val>(q);
   const uint32_t c     = q.w >> SPB200_IDX_BITS;
-  acc[N - 2]           = fma2(v, b, acc[N - 2]);
+  acc[N - 2]           = vfma(v, b, acc[N - 2]);
   if (c) {
-    acc[N - 3] = fma2(acc[N - 2], r, acc[N - 3]);
+    acc[N - 3] = vfma(acc[N - 2], r, acc[N - 3]);
     acc[N - 2] = zero2;
     if (c >= 2) {
       if constexpr (N >= 4) {
         ++pos[N - 3];
-        acc[N - 4] = fma2(acc[N - 3], r2, acc[N - 4]);
+        acc[N - 4] = vfma(acc[N - 3], r2, acc[N - 4]);
         acc[N - 3] = zero2;
 #pragma unroll
         for (int l = N - 4; l >= 1; --l) {
           if (c >= uint32_t(N - 1 - l)) {
             const uint32_t idx = __ldg(&a.up[l][pos[l]]);
             ++pos[l];
-            acc[l - 1] = fma2(acc[l], ld_row(mbase[l], idx, pitch), acc[l - 1]);
+            acc[l - 1] = vfma(acc[l], ld_row<V>(mbase[l], idx, pitch), acc[l - 1]);
             acc[l]     = zero2;
           }
         }
@@ -208,11 +259,17 @@ __device__ __forceinline__ void root_record(const MttkrpArgs & a, const uint4 q,
   }
 }
 
-template <int N, int L, int KIND, int BATCH, bool KT, bool MC, int MINB = ((BATCH >= 8 || N >= 4) ? 2 : 3),
-          int STAGES = kStages>
-__global__ void __launch_bounds__(kThreads, MINB)
+// Val: value type of the factors, the output and the arithmetic (double or float).  The
+// records are the same for both: an fp32 kernel rounds each record's fp64 value once.
+// MAXREG: register limit on top of the one MINB implies (the tighter applies); 255 = none.
+template <typename Val, int N, int L, int KIND, int BATCH, bool KT, bool MC,
+          int MINB = default_minb(N, BATCH), int STAGES = kStages, int MAXREG = 255>
+__global__ void __launch_bounds__(kThreads, MINB) __maxnreg__(MAXREG)
 mttkrp_stream_kernel(const MttkrpArgs a) {
   static_assert(N >= 2 && N <= SPB200_MAXN, "2..8 modes");
+  static_assert(!MC || sizeof(Val) == 8, "multicast output is fp64 only");
+  using V          = typename LaneVec<Val>::type;
+  constexpr int W  = LaneVec<Val>::W;     // columns per lane
   constexpr int G  = 32 / L;            // groups per warp
   constexpr int SU = kStageRecs / G;    // records per group per stage
   constexpr int kStages = STAGES;       // shadows the namespace default inside the kernel
@@ -232,9 +289,9 @@ mttkrp_stream_kernel(const MttkrpArgs a) {
   const int      lane   = threadIdx.x & 31;
   const int      grp    = lane / L;
   const int      gl     = lane % L;
-  const bool     act    = (2 * gl) < a.ncols;   // lanes past the last column only keep the warp in step
+  const bool     act    = (W * gl) < a.ncols;   // lanes past the last column only keep the warp in step
   const bool     leader = (gl == 0);
-  const uint32_t pitch  = static_cast<uint32_t>(a.ldm) * 8u;
+  const uint32_t pitch  = static_cast<uint32_t>(a.ldm) * static_cast<uint32_t>(sizeof(Val));
 
   if (lane == 0) {
 #pragma unroll
@@ -282,18 +339,18 @@ mttkrp_stream_kernel(const MttkrpArgs a) {
     }
   };
 
-  // Per-lane matrix bases (already offset to this lane's column pair), by level.
-  const int    colx = act ? (a.col0 + 2 * gl) : a.col0;
+  // Per-lane matrix bases (already offset to this lane's columns), by level.
+  const int    colx = act ? (a.col0 + W * gl) : a.col0;
   const char * mbase[N];
 #pragma unroll
-  for (int l = 0; l < N; ++l) mbase[l] = reinterpret_cast<const char *>(a.mats[l] + colx);
-  char * obase = reinterpret_cast<char *>(a.out + colx);
+  for (int l = 0; l < N; ++l) mbase[l] = reinterpret_cast<const char *>(static_cast<const Val *>(a.mats[l]) + colx);
+  char * obase = reinterpret_cast<char *>(static_cast<Val *>(a.out) + colx);
 
   // Traversal state.
-  const double2 zero2 = make_double2(0.0, 0.0);
+  const V       zero2 = vzero<V>();
   constexpr int NP = (N > 2) ? N - 2 : 1;
-  double2       acc[N - 1];   // partial sums of levels 0..N-2 (levels >= outdepth)
-  double2       pre[N - 1];   // Hadamard prefixes of levels 0..N-2 (levels < outdepth)
+  V             acc[N - 1];   // partial sums of levels 0..N-2 (levels >= outdepth)
+  V             pre[N - 1];   // Hadamard prefixes of levels 0..N-2 (levels < outdepth)
   uint32_t      pos[NP];      // current node at levels 0..N-3
 #pragma unroll
   for (int l = 0; l < N - 1; ++l) { acc[l] = zero2; pre[l] = zero2; }
@@ -329,18 +386,18 @@ mttkrp_stream_kernel(const MttkrpArgs a) {
         // reference: the generic kernels with nmodes == 2, src/mttkrp.c:668-732 / :860-943.
         for (uint32_t n = 0; n < cnt; ++n) {
           const uint4    q   = *reinterpret_cast<const uint4 *>(&buf[n]);
-          const double   v   = __hiloint2double(static_cast<int>(q.y), static_cast<int>(q.x));
+          const Val      v   = rec_val<Val>(q);
           const uint32_t par = q.w & SPB200_IDX_MASK;
           if constexpr (KIND == SPB200_KIND_ROOT) {
-            acc[0] = fma2(v, ld_row(mbase[1], q.z, pitch), acc[0]);
+            acc[0] = vfma(v, ld_row<V>(mbase[1], q.z, pitch), acc[0]);
             if (q.w >> SPB200_IDX_BITS) {
               if constexpr (MC) red_row_mc(obase, par, pitch, acc[0]);
               else red_row(obase, par, pitch, acc[0]);
               acc[0] = zero2;
             }
           } else {
-            const double2 row = ld_row(mbase[0], par, pitch);
-            red_row(obase, q.z, pitch, make_double2(v * row.x, v * row.y));
+            const V row = ld_row<V>(mbase[0], par, pitch);
+            red_row(obase, q.z, pitch, vmul(v, row));
           }
         }
       } else if constexpr (KIND == SPB200_KIND_ROOT) {
@@ -348,7 +405,7 @@ mttkrp_stream_kernel(const MttkrpArgs a) {
         // full batches: all gathers of BATCH records are in flight before the first FMA
         for (; n0 + BATCH <= cnt; n0 += BATCH) {
           uint4    q[BATCH];
-          double2  b[BATCH], r[BATCH], r2[BATCH];
+          V        b[BATCH], r[BATCH], r2[BATCH];
           uint32_t hi = 0;
 #pragma unroll
           for (int u = 0; u < BATCH; ++u) {
@@ -356,12 +413,12 @@ mttkrp_stream_kernel(const MttkrpArgs a) {
             hi   = max(hi, q[u].w);
           }
 #pragma unroll
-          for (int u = 0; u < BATCH; ++u) b[u] = ld_row(mbase[N - 1], q[u].z, pitch);
+          for (int u = 0; u < BATCH; ++u) b[u] = ld_row<V>(mbase[N - 1], q[u].z, pitch);
 #pragma unroll
           for (int u = 0; u < BATCH; ++u)
             if (q[u].w >> SPB200_IDX_BITS)
-              r[u] = KT ? ld_row_na(mbase[N - 2], q[u].w & SPB200_IDX_MASK, pitch)
-                        : ld_row(mbase[N - 2], q[u].w & SPB200_IDX_MASK, pitch);
+              r[u] = KT ? ld_row_na<V>(mbase[N - 2], q[u].w & SPB200_IDX_MASK, pitch)
+                        : ld_row<V>(mbase[N - 2], q[u].w & SPB200_IDX_MASK, pitch);
           uint32_t p2 = 0;
           if constexpr (N >= 4) {
             // level N-3 closes are frequent on deep trees; the id of the closing node rides
@@ -370,7 +427,7 @@ mttkrp_stream_kernel(const MttkrpArgs a) {
 #pragma unroll
             for (int u = 0; u < BATCH; ++u)
               if ((q[u].w >> SPB200_IDX_BITS) >= 2u) {
-                r2[u] = ld_row(mbase[N - 3], abuf[n0 + u], pitch);
+                r2[u] = ld_row<V>(mbase[N - 3], abuf[n0 + u], pitch);
                 ++p2;
               }
           }
@@ -380,16 +437,16 @@ mttkrp_stream_kernel(const MttkrpArgs a) {
             // batch -- straight-line, predicated, no branches
 #pragma unroll
             for (int u = 0; u < BATCH; ++u) {
-              const double   v = __hiloint2double(static_cast<int>(q[u].y), static_cast<int>(q[u].x));
+              const Val      v = rec_val<Val>(q[u]);
               const uint32_t c = q[u].w >> SPB200_IDX_BITS;
-              acc[N - 2]       = fma2(v, b[u], acc[N - 2]);
+              acc[N - 2]       = vfma(v, b[u], acc[N - 2]);
               if (c) {
-                acc[N - 3] = fma2(acc[N - 2], r[u], acc[N - 3]);
+                acc[N - 3] = vfma(acc[N - 2], r[u], acc[N - 3]);
                 acc[N - 2] = zero2;
               }
               if constexpr (N >= 4) {
                 if (c >= 2u) {
-                  acc[N - 4] = fma2(acc[N - 3], r2[u], acc[N - 4]);
+                  acc[N - 4] = vfma(acc[N - 3], r2[u], acc[N - 4]);
                   acc[N - 3] = zero2;
                 }
               }
@@ -398,40 +455,40 @@ mttkrp_stream_kernel(const MttkrpArgs a) {
           } else {
 #pragma unroll
             for (int u = 0; u < BATCH; ++u)
-              root_record<N, MC>(a, q[u], b[u], r[u], r2[u], acc, pos, mbase, obase, pitch, seen_root,
+              root_record<Val, N, MC>(a, q[u], b[u], r[u], r2[u], acc, pos, mbase, obase, pitch, seen_root,
                                  off + n0 + u + 1 == T);
           }
         }
         for (; n0 < cnt; ++n0) {   // tail of the range's last stage
           const uint4   q = *reinterpret_cast<const uint4 *>(&buf[n0]);
-          const double2 b = ld_row(mbase[N - 1], q.z, pitch);
-          double2       r = zero2, r2 = zero2;
-          if (q.w >> SPB200_IDX_BITS) r = ld_row(mbase[N - 2], q.w & SPB200_IDX_MASK, pitch);
+          const V       b = ld_row<V>(mbase[N - 1], q.z, pitch);
+          V             r = zero2, r2 = zero2;
+          if (q.w >> SPB200_IDX_BITS) r = ld_row<V>(mbase[N - 2], q.w & SPB200_IDX_MASK, pitch);
           if constexpr (N >= 4) {
-            if ((q.w >> SPB200_IDX_BITS) >= 2u) r2 = ld_row(mbase[N - 3], abuf[n0], pitch);
+            if ((q.w >> SPB200_IDX_BITS) >= 2u) r2 = ld_row<V>(mbase[N - 3], abuf[n0], pitch);
           }
-          root_record<N, MC>(a, q, b, r, r2, acc, pos, mbase, obase, pitch, seen_root, off + n0 + 1 == T);
+          root_record<Val, N, MC>(a, q, b, r, r2, acc, pos, mbase, obase, pitch, seen_root, off + n0 + 1 == T);
         }
       } else if constexpr (KIND == SPB200_KIND_INTL) {
 #pragma unroll 2
         for (uint32_t n = 0; n < cnt; ++n) {
           const uint4    q   = *reinterpret_cast<const uint4 *>(&buf[n]);
-          const double   v   = __hiloint2double(static_cast<int>(q.y), static_cast<int>(q.x));
+          const Val      v   = rec_val<Val>(q);
           const uint32_t c   = q.w >> SPB200_IDX_BITS;
           const uint32_t par = q.w & SPB200_IDX_MASK;
-          const double2  b   = ld_row(mbase[N - 1], q.z, pitch);
+          const V        b   = ld_row<V>(mbase[N - 1], q.z, pitch);
           // (re)open prefix levels that changed after the previous record
           if (pc >= uint32_t(N - d)) {
 #pragma unroll
             for (int l = 0; l <= N - 3; ++l) {
               if (l < d && l + int(pc) >= N - 1) {
                 const uint32_t idx = __ldg(&a.up[l][pos[l]]);
-                const double2  row = ld_row(mbase[l], idx, pitch);
-                pre[l]             = (l == 0) ? row : mul2(pre[l - 1], row);
+                const V        row = ld_row<V>(mbase[l], idx, pitch);
+                pre[l]             = (l == 0) ? row : vmul(pre[l - 1], row);
               }
             }
           }
-          acc[N - 2] = fma2(v, b, acc[N - 2]);
+          acc[N - 2] = vfma(v, b, acc[N - 2]);
           if (c) {
             // levels below the output level fold upwards
 #pragma unroll
@@ -440,7 +497,7 @@ mttkrp_stream_kernel(const MttkrpArgs a) {
                 uint32_t idx;
                 if (l == N - 2) idx = par;
                 else { idx = __ldg(&a.up[l][pos[l]]); ++pos[l]; }
-                acc[l - 1] = fma2(acc[l], ld_row(mbase[l], idx, pitch), acc[l - 1]);
+                acc[l - 1] = vfma(acc[l], ld_row<V>(mbase[l], idx, pitch), acc[l - 1]);
                 acc[l]     = zero2;
               }
             }
@@ -451,7 +508,7 @@ mttkrp_stream_kernel(const MttkrpArgs a) {
                 uint32_t idx;
                 if (l == N - 2) idx = par;
                 else { idx = __ldg(&a.up[l][pos[l]]); ++pos[l]; }
-                red_row(obase, idx, pitch, mul2(pre[l - 1], acc[l]));
+                red_row(obase, idx, pitch, vmul(pre[l - 1], acc[l]));
                 acc[l] = zero2;
               }
             }
@@ -466,7 +523,7 @@ mttkrp_stream_kernel(const MttkrpArgs a) {
 #pragma unroll 2
         for (uint32_t n = 0; n < cnt; ++n) {
           const uint4    q   = *reinterpret_cast<const uint4 *>(&buf[n]);
-          const double   v   = __hiloint2double(static_cast<int>(q.y), static_cast<int>(q.x));
+          const Val      v   = rec_val<Val>(q);
           const uint32_t c   = q.w >> SPB200_IDX_BITS;
           const uint32_t par = q.w & SPB200_IDX_MASK;
           if (pc) {
@@ -476,12 +533,12 @@ mttkrp_stream_kernel(const MttkrpArgs a) {
                 uint32_t idx;
                 if (l == N - 2) idx = par;
                 else idx = __ldg(&a.up[l][pos[l]]);
-                const double2 row = ld_row(mbase[l], idx, pitch);
-                pre[l]            = (l == 0) ? row : mul2(pre[l - 1], row);
+                const V       row = ld_row<V>(mbase[l], idx, pitch);
+                pre[l]            = (l == 0) ? row : vmul(pre[l - 1], row);
               }
             }
           }
-          red_row(obase, q.z, pitch, make_double2(v * pre[N - 2].x, v * pre[N - 2].y));
+          red_row(obase, q.z, pitch, vmul(v, pre[N - 2]));
           if (c) {
 #pragma unroll
             for (int l = 0; l <= N - 3; ++l)

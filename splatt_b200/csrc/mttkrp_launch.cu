@@ -1,6 +1,7 @@
 // Host-side dispatch of one MTTKRP over a fiber stream.
 #include "common.h"
 #include <cstdlib>
+#include <type_traits>
 
 unsigned long long g_spb200_launches = 0;
 unsigned long long g_spb200_builds = 0;
@@ -34,6 +35,13 @@ int launch_n5(int, const MttkrpArgs &, int, cudaStream_t);
 int launch_n6(int, const MttkrpArgs &, int, cudaStream_t);
 int launch_n7(int, const MttkrpArgs &, int, cudaStream_t);
 int launch_n8(int, const MttkrpArgs &, int, cudaStream_t);
+int launch_f32_n2(int, const MttkrpArgs &, int, cudaStream_t);
+int launch_f32_n3(int, const MttkrpArgs &, int, cudaStream_t);
+int launch_f32_n4(int, const MttkrpArgs &, int, cudaStream_t);
+int launch_f32_n5(int, const MttkrpArgs &, int, cudaStream_t);
+int launch_f32_n6(int, const MttkrpArgs &, int, cudaStream_t);
+int launch_f32_n7(int, const MttkrpArgs &, int, cudaStream_t);
+int launch_f32_n8(int, const MttkrpArgs &, int, cudaStream_t);
 }  // namespace spb200
 
 static int num_sms_of_current_device() {
@@ -49,23 +57,34 @@ static int num_sms_of_current_device() {
   return cached[dev];
 }
 
-int spb200_launch_mttkrp(const FiberStream & s, int kind, int outdepth, int ncolumns, int ldm,
-                         const double * const * d_mats_by_mode, double * d_out,
+// T = double or float.  A lane moves 16 bytes of a row, i.e. W = 16 / sizeof(T) columns: ldm,
+// the padded rank and column blocks are multiples of W, and one launch covers 32 * W columns.
+template <typename T>
+static int launch_mttkrp(const FiberStream & s, int kind, int outdepth, int ncolumns, int ldm,
+                         const T * const * d_mats_by_mode, T * d_out,
                          uint64_t out_rows, cudaStream_t stream, bool multicast_out,
                          int col_begin, int col_count, const GroupSync * sync) {
+  constexpr int W    = 16 / static_cast<int>(sizeof(T));
+  constexpr int kCol = 32 * W;        // columns per launch (L = 32)
   const int N = s.nmodes;
   if (N < 2 || N > SPB200_MAXN) {
     fprintf(stderr, "SPLATT: MTTKRP supports 2..%d modes (got %d)\n", SPB200_MAXN, N);
     return SPLATT_ERROR_BADINPUT;
   }
-  if (ncolumns <= 0 || ldm < ncolumns + (ncolumns & 1) || (ldm & 1)) {
-    fprintf(stderr, "SPLATT: bad ncolumns/ldm (%d/%d): ldm must be even and >= ncolumns\n",
-            ncolumns, ldm);
+  // padded rank: ncolumns rounded up to a whole lane vector
+  const int rpad_all = (ncolumns + W - 1) & ~(W - 1);
+  if (ncolumns <= 0 || ldm < rpad_all || (ldm & (W - 1))) {
+    if (W == 2)
+      fprintf(stderr, "SPLATT: bad ncolumns/ldm (%d/%d): ldm must be even and >= ncolumns\n",
+              ncolumns, ldm);
+    else
+      fprintf(stderr, "SPLATT: bad ncolumns/ldm (%d/%d): ldm must be a multiple of %d and >= ncolumns\n",
+              ncolumns, ldm, W);
     return SPLATT_ERROR_BADINPUT;
   }
   // rows are fetched with 128-bit loads: every matrix base must be 16-byte aligned
   for (int m = 0; m < N; ++m) {
-    const double * p = d_mats_by_mode[m];
+    const T * p = d_mats_by_mode[m];
     if (p && (reinterpret_cast<uintptr_t>(p) & 15u)) {
       fprintf(stderr, "SPLATT: factor matrix %d is not 16-byte aligned\n", m);
       return SPLATT_ERROR_BADINPUT;
@@ -82,36 +101,38 @@ int spb200_launch_mttkrp(const FiberStream & s, int kind, int outdepth, int ncol
       return SPLATT_ERROR_BADINPUT;
     }
   }
-  const int rpad_all = ncolumns + (ncolumns & 1);
   if (col_count <= 0) { col_begin = 0; col_count = rpad_all; }        // whole matrix
-  // an odd block is widened to the next even column, which must still lie inside rpad_all:
+  // a block is widened to the next multiple of W, which must still lie inside rpad_all:
   // past it the zeroing and the kernel would reach into the next row (or past the buffer)
-  if ((col_begin & 1) || col_begin < 0 || col_count > rpad_all - col_begin ||
+  if ((col_begin & (W - 1)) || col_begin < 0 || col_count > rpad_all - col_begin ||
       col_begin >= rpad_all) {
     fprintf(stderr, "SPLATT: bad column block [%d, %d) of %d\n", col_begin, col_begin + col_count,
             rpad_all);
     return SPLATT_ERROR_BADINPUT;
   }
-  const int col_end = (col_begin + col_count + 1) & ~1;               // even, <= rpad_all
+  const int col_end = (col_begin + col_count + W - 1) & ~(W - 1);     // <= rpad_all
   if (!multicast_out) {
     if (col_begin == 0 && col_end == rpad_all)
-      SPB200_CUDA_OK(cudaMemsetAsync(d_out, 0, sizeof(double) * out_rows * ldm, stream));
+      SPB200_CUDA_OK(cudaMemsetAsync(d_out, 0, sizeof(T) * out_rows * ldm, stream));
     else
-      SPB200_CUDA_OK(cudaMemset2DAsync(d_out + col_begin, sizeof(double) * ldm, 0,
-                                       sizeof(double) * (col_end - col_begin), out_rows, stream));
+      SPB200_CUDA_OK(cudaMemset2DAsync(d_out + col_begin, sizeof(T) * ldm, 0,
+                                       sizeof(T) * (col_end - col_begin), out_rows, stream));
   }
   if (s.nrec == 0 && !(multicast_out && sync)) return SPLATT_SUCCESS;
 
-  // leaf factor staged in shared memory (CTA-tiled stream, 3-mode root)
-  if (!multicast_out && spb200_tiled_applicable(s, kind)) {
-    static int use_tiled = -1;
-    if (use_tiled < 0) {
-      const char * e = getenv("SPLATT_B200_TILED_KERNEL");
-      use_tiled = (e && atoi(e) == 0) ? 0 : 1;
+  // leaf factor staged in shared memory (CTA-tiled stream, 3-mode root).  That kernel is fp64
+  // only: an fp32 call on such a stream runs the generic kernel (leaf-tiled variant).
+  if constexpr (std::is_same<T, double>::value) {
+    if (!multicast_out && spb200_tiled_applicable(s, kind)) {
+      static int use_tiled = -1;
+      if (use_tiled < 0) {
+        const char * e = getenv("SPLATT_B200_TILED_KERNEL");
+        use_tiled = (e && atoi(e) == 0) ? 0 : 1;
+      }
+      if (use_tiled)
+        return spb200_launch_tiled_root3(s, ldm, col_begin, col_end, d_mats_by_mode[s.perm[2]],
+                                         d_mats_by_mode[s.perm[1]], d_out, stream);
     }
-    if (use_tiled)
-      return spb200_launch_tiled_root3(s, ldm, col_begin, col_end, d_mats_by_mode[s.perm[2]],
-                                       d_mats_by_mode[s.perm[1]], d_out, stream);
   }
 
   MttkrpArgs a;
@@ -155,28 +176,43 @@ int spb200_launch_mttkrp(const FiberStream & s, int kind, int outdepth, int ncol
     a.mc_store = (mc_store && !s.ktile_rows) ? 1 : 0;
   }
 
+  using Launch = int (*)(int, const MttkrpArgs &, int, cudaStream_t);
+  static constexpr Launch kLaunch[] = {spb200::launch_n2, spb200::launch_n3, spb200::launch_n4,
+                                       spb200::launch_n5, spb200::launch_n6, spb200::launch_n7,
+                                       spb200::launch_n8};
+  static constexpr Launch kLaunchF32[] = {spb200::launch_f32_n2, spb200::launch_f32_n3,
+                                          spb200::launch_f32_n4, spb200::launch_f32_n5,
+                                          spb200::launch_f32_n6, spb200::launch_f32_n7,
+                                          spb200::launch_f32_n8};
+  const Launch launch = (std::is_same<T, double>::value ? kLaunch : kLaunchF32)[N - 2];
   const int num_sms = num_sms_of_current_device();
-  for (int c0 = col_begin; c0 < col_end; c0 += 64) {
+  for (int c0 = col_begin; c0 < col_end; c0 += kCol) {
     a.col0  = c0;
-    a.ncols = (col_end - c0 < 64) ? (col_end - c0) : 64;
-    if (multicast_out && sync && c0 + 64 >= col_end) {     // the last column pass carries the barrier
+    a.ncols = (col_end - c0 < kCol) ? (col_end - c0) : kCol;
+    if (multicast_out && sync && c0 + kCol >= col_end) {   // the last column pass carries the barrier
       a.sync_mc = sync->mc_flag; a.sync_local = sync->local_flag; a.sync_cta = sync->cta_done;
       a.sync_target = sync->target;
       a.sync_rank = sync->rank; a.sync_world = sync->world;
     }
-    int rc;
-    switch (N) {
-      case 2:  rc = spb200::launch_n2(kind, a, num_sms, stream); break;
-      case 3:  rc = spb200::launch_n3(kind, a, num_sms, stream); break;
-      case 4:  rc = spb200::launch_n4(kind, a, num_sms, stream); break;
-      case 5:  rc = spb200::launch_n5(kind, a, num_sms, stream); break;
-      case 6:  rc = spb200::launch_n6(kind, a, num_sms, stream); break;
-      case 7:  rc = spb200::launch_n7(kind, a, num_sms, stream); break;
-      default: rc = spb200::launch_n8(kind, a, num_sms, stream); break;
-    }
+    const int rc = launch(kind, a, num_sms, stream);
     if (rc != SPLATT_SUCCESS) return rc;
   }
   return SPLATT_SUCCESS;
+}
+
+int spb200_launch_mttkrp(const FiberStream & s, int kind, int outdepth, int ncolumns, int ldm,
+                         const double * const * d_mats_by_mode, double * d_out,
+                         uint64_t out_rows, cudaStream_t stream, bool multicast_out,
+                         int col_begin, int col_count, const GroupSync * sync) {
+  return launch_mttkrp<double>(s, kind, outdepth, ncolumns, ldm, d_mats_by_mode, d_out, out_rows,
+                               stream, multicast_out, col_begin, col_count, sync);
+}
+
+int spb200_launch_mttkrp_f32(const FiberStream & s, int kind, int outdepth, int ncolumns, int ldm,
+                             const float * const * d_mats_by_mode, float * d_out,
+                             uint64_t out_rows, cudaStream_t stream) {
+  return launch_mttkrp<float>(s, kind, outdepth, ncolumns, ldm, d_mats_by_mode, d_out, out_rows,
+                              stream, false, 0, 0, nullptr);
 }
 
 

@@ -245,11 +245,11 @@ __global__ void __launch_bounds__(kTW * 32, 1) mttkrp_tiled_root3(const TiledArg
           for (int u = 0; u < kTB; ++u) {
             const uint4  q = *reinterpret_cast<const uint4 *>(&bq[u]);
             const double v = __hiloint2double(static_cast<int>(q.y), static_cast<int>(q.x));
-            acc1           = fma2(v, lds_f64x2(tile + q.z * a.tpitch), acc1);
+            acc1           = vfma(v, lds_f64x2(tile + q.z * a.tpitch), acc1);
             if (u + 1 < kTB && ((cc >> (8 * u)) & 0xffu)) { p[u] = acc1; acc1 = zero2; }
           }
           auto close = [&](int u) {
-            acc0 = fma2(u + 1 < kTB ? p[u] : acc1, r[u], acc0);
+            acc0 = vfma(u + 1 < kTB ? p[u] : acc1, r[u], acc0);
             if (u + 1 == kTB) acc1 = zero2;
           };
           if ((cc & 0xfefefefeu) == 0) {             // no slice ends in the batch
@@ -273,9 +273,9 @@ __global__ void __launch_bounds__(kTW * 32, 1) mttkrp_tiled_root3(const TiledArg
           const double   v = __hiloint2double(static_cast<int>(q.y), static_cast<int>(q.x));
           const uint32_t c = q.w >> SPB200_IDX_BITS;
           const double2  b = lds_f64x2(tile + q.z * a.tpitch);
-          acc1             = fma2(v, b, acc1);
+          acc1             = vfma(v, b, acc1);
           if (c) {
-            acc0 = fma2(acc1, ld_row_na(reinterpret_cast<const char *>(a.parent) + poff, q.w & SPB200_IDX_MASK, pitch), acc0);
+            acc0 = vfma(acc1, ld_row_na(reinterpret_cast<const char *>(a.parent) + poff, q.w & SPB200_IDX_MASK, pitch), acc0);
             acc1 = zero2;
             if (c >= 2) flush(n);
           }
