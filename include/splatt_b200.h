@@ -505,6 +505,57 @@ int  splatt_b200_als_tail_update(splatt_b200_als_tail * h, int mode, double cons
 int  splatt_b200_als_tail_fit(splatt_b200_als_tail * h, double const * d_last_factor,
                               double const * d_last_m1, uint64_t rows, double ttnormsq,
                               double * fit_out, double * lambda_out);
+/* The same three steps with fp32 factors and an fp32 M1 (the output of splatt_b200_mttkrp_f32),
+ * on the same handle.  Grams, the normal matrix, its Cholesky factor or pseudo-inverse, lambda,
+ * the fit's inner product and the fit stay fp64; each row is solved in fp64 from its fp32 values
+ * and rounded to fp32 once, and the column scaling is done in fp64 and rounded once.  Columns
+ * [ncolumns, ldm) of d_m1 never feed the results (they may hold anything, NaN included; the
+ * row solve loads whole float4 groups and discards those columns by selection), and columns
+ * [ncolumns, ldm) of d_factor are never written.  Needs a handle created with ldm % 4 == 0 and
+ * 16-byte aligned matrices; otherwise SPLATT_ERROR_BADINPUT and nothing is enqueued. */
+int  splatt_b200_als_tail_gram_f32(splatt_b200_als_tail * h, int mode, float const * d_factor,
+                                   uint64_t rows);
+int  splatt_b200_als_tail_update_f32(splatt_b200_als_tail * h, int mode, float const * d_m1,
+                                     float * d_factor, uint64_t rows, int first_iteration);
+int  splatt_b200_als_tail_fit_f32(splatt_b200_als_tail * h, float const * d_last_factor,
+                                  float const * d_last_m1, uint64_t rows, double ttnormsq,
+                                  double * fit_out, double * lambda_out);
+
+/* CPD-ALS of a device-resident tensor from device-resident factors (no host CSF, no host
+ * factors): the iteration of splatt_cpd_als with the dense tail on the device, then its
+ * post-processing.
+ *   d_factors[m]  dims[m] x ldm, row-major, in/out.  On entry the caller's initial factors; on
+ *                 return the 2-normalised factors.  Columns [ncolumns, ldm) never feed the
+ *                 results and are never written (they may be read: the MTTKRP loads rows in
+ *                 16-byte groups, up to column (ncolumns + 3) & ~3 in fp32).
+ *   lambda_out    ncolumns host doubles: the weights (may be NULL).
+ *   fit_out       the fit of the last iteration (may be NULL).
+ *   iterations_out the number of iterations run (may be NULL).
+ * Reads options[SPLATT_OPTION_NITER], [SPLATT_OPTION_TOLERANCE] and [SPLATT_OPTION_VERBOSITY]
+ * and stops as splatt_cpd_als does: after NITER iterations, at fit == 1, or when the fit moved
+ * by less than TOLERANCE (from the second iteration on).  ||X||^2 is summed from the tensor's
+ * own values.  Runs on t->device and enqueues on `stream` (a cudaStream_t; NULL = default
+ * stream); synchronises the stream once before the first iteration (||X||^2), once per
+ * iteration (the fit) and once at the end.
+ * Input rules: 1 <= ncolumns <= 128; fp64: ldm even and >= ncolumns; fp32: ldm % 4 == 0 and
+ * ldm >= (ncolumns + 3) & ~3; every d_factors[m] 16-byte aligned; the tensor is whole (built
+ * with shard_count <= 1: a shard's values are only a part of ||X||^2).  A violation returns
+ * SPLATT_ERROR_BADINPUT before anything is enqueued, and the factors are left untouched.
+ * _f32: factors and MTTKRP in fp32 (splatt_b200_mttkrp_f32), the dense tail as in
+ * splatt_b200_als_tail_update_f32.  The fit's inner product <X,K> is formed from the fp32
+ * MTTKRP result, and the fit 1 - sqrt(||X||^2 + ||K||^2 - 2<X,K>) / ||X|| cancels digits as it
+ * approaches 1: there it is resolved only to about sqrt(2 eps) for a relative error eps in <X,K>
+ * (about 1e-4 on a dense 30^3 tensor of exact rank 3, where fp64 reaches 1.0).  Near such a fit
+ * the fp32 fit moves by about that much from one iteration to the next, so a TOLERANCE below it
+ * may never stop the run before NITER. */
+int splatt_b200_cpd_als_device(splatt_b200_tensor const * t, int ncolumns, int ldm,
+                               double const * options, double * const * d_factors,
+                               double * lambda_out, double * fit_out, int * iterations_out,
+                               void * stream);
+int splatt_b200_cpd_als_device_f32(splatt_b200_tensor const * t, int ncolumns, int ldm,
+                                   double const * options, float * const * d_factors,
+                                   double * lambda_out, double * fit_out, int * iterations_out,
+                                   void * stream);
 
 /* Measurement aid: a pure gather kernel with the MTTKRP's access pattern (whole
  * fp64 rows of a rows x ldm matrix at d_idx[0..nidx), 128-bit loads, eight rows in

@@ -100,6 +100,8 @@ EXPORTS = [
     "splatt_b200_version", "splatt_b200_level_orders", "splatt_b200_cta_tiling", "splatt_b200_shard_range", "splatt_b200_mttkrp_multicast", "splatt_b200_gather_probe", "splatt_b200_gather_probe_ex", "splatt_b200_mttkrp_columns",
     "splatt_b200_als_tail_create", "splatt_b200_als_tail_free", "splatt_b200_als_tail_gram",
     "splatt_b200_als_tail_update", "splatt_b200_als_tail_fit", "splatt_b200_csf_to_coo",
+    "splatt_b200_als_tail_gram_f32", "splatt_b200_als_tail_update_f32",
+    "splatt_b200_als_tail_fit_f32", "splatt_b200_cpd_als_device", "splatt_b200_cpd_als_device_f32",
     "splatt_b200_tensor_shard", "splatt_b200_mttkrp_multicast_sync",
     "splatt_b200_mttkrp_multicast_sync_columns",
     "splatt_b200_multi_env_devices", "splatt_b200_multi_create", "splatt_b200_multi_free",
@@ -187,6 +189,23 @@ def load() -> C.CDLL:
     lib.splatt_b200_als_tail_fit.restype = C.c_int
     lib.splatt_b200_als_tail_fit.argtypes = [C.c_void_p, val_p, val_p, C.c_uint64, C.c_double,
                                              C.POINTER(C.c_double), val_p]
+    lib.splatt_b200_als_tail_gram_f32.restype = C.c_int
+    lib.splatt_b200_als_tail_gram_f32.argtypes = [C.c_void_p, C.c_int, f32_p, C.c_uint64]
+    lib.splatt_b200_als_tail_update_f32.restype = C.c_int
+    lib.splatt_b200_als_tail_update_f32.argtypes = [C.c_void_p, C.c_int, f32_p, f32_p, C.c_uint64,
+                                                    C.c_int]
+    lib.splatt_b200_als_tail_fit_f32.restype = C.c_int
+    lib.splatt_b200_als_tail_fit_f32.argtypes = [C.c_void_p, f32_p, f32_p, C.c_uint64, C.c_double,
+                                                 C.POINTER(C.c_double), val_p]
+    lib.splatt_b200_cpd_als_device.restype = C.c_int
+    lib.splatt_b200_cpd_als_device.argtypes = [C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_double),
+                                               vpp, val_p, C.POINTER(C.c_double),
+                                               C.POINTER(C.c_int), C.c_void_p]
+    lib.splatt_b200_cpd_als_device_f32.restype = C.c_int
+    lib.splatt_b200_cpd_als_device_f32.argtypes = [C.c_void_p, C.c_int, C.c_int,
+                                                   C.POINTER(C.c_double), C.POINTER(f32_p), val_p,
+                                                   C.POINTER(C.c_double), C.POINTER(C.c_int),
+                                                   C.c_void_p]
     lib.splatt_b200_csf_to_coo.restype = C.c_int
     lib.splatt_b200_csf_to_coo.argtypes = [csf_p, u32pp, val_p]
     lib.splatt_b200_gather_probe.restype = C.c_int

@@ -328,6 +328,72 @@ class Tensor:
         _check(rc, sym)
         return out
 
+    def cpd_als(self, rank: int, factors=None, *, dtype=None, niters: int = 50, tol: float = 1e-5,
+                seed: int = 0, verbosity: int = 0, stream=None):
+        """CPD-ALS of this (whole) tensor on its device (splatt_b200_cpd_als_device, or _f32 for
+        float32: fp32 factors and MTTKRP, fp64 Grams, solves, lambda and fit).  The tensor must
+        live on the current CUDA device, as for Tensor.mttkrp: the start buffers and the default
+        stream are taken from it.
+
+        factors: list of CUDA tensors (dims[m] x rank) of one dtype, the start; copied into
+        padded buffers, never written.  None: uniform on [-3, 3) (the reference's rand_val range)
+        from a torch.Generator seeded with `seed`, in `dtype` (default float64).  Stops after
+        `niters` iterations or when the fit moves by less than `tol`.  In float32 the fit is
+        formed from the fp32 MTTKRP result and, close to 1, resolved only to about 1e-4 (see
+        splatt_b200_cpd_als_device_f32 in include/splatt_b200.h): a `tol` below that may not stop
+        the run before `niters` there.
+        Returns (fit, lambda (numpy float64[rank]), factors (2-normalised, CUDA views
+        dims[m] x rank), iterations)."""
+        import torch
+        if factors is not None:
+            dt = factors[0].dtype
+            if dtype is not None and dtype != dt:
+                raise ValueError(f"factor matrix 0 is {dt} but dtype is {dtype}")
+            for m, f in enumerate(factors):
+                if f.dtype != dt:
+                    raise ValueError(f"factor matrix {m} is {f.dtype} but factor matrix 0 is {dt}")
+            if len(factors) != self.nmodes:
+                raise ValueError(f"{len(factors)} factor matrices for a {self.nmodes}-mode tensor")
+        dev = torch.device("cuda", torch.cuda.current_device())
+        if factors is not None:
+            for m, f in enumerate(factors):
+                if f.device != dev or tuple(f.shape) != (self.dims[m], rank):
+                    raise ValueError(f"factor matrix {m} must be a tensor of shape "
+                                     f"({self.dims[m]}, {rank}) on the current device {dev}")
+        else:
+            dt = torch.float64 if dtype is None else dtype
+        if dt == torch.float64:
+            ptr_t, sym, ldm = A.val_p, "splatt_b200_cpd_als_device", rank + (rank & 1)
+        elif dt == torch.float32:
+            ptr_t, sym, ldm = A.f32_p, "splatt_b200_cpd_als_device_f32", (rank + 3) & ~3
+        else:
+            raise ValueError(f"CPD factors must be float64 or float32, not {dt}")
+        bufs = [torch.zeros((d, ldm), dtype=dt, device=dev) for d in self.dims]
+        if factors is None:
+            g = torch.Generator(device=dev).manual_seed(seed)
+            for b in bufs:
+                b[:, :rank].uniform_(-3.0, 3.0, generator=g)
+        else:
+            for b, f in zip(bufs, factors):
+                b[:, :rank].copy_(f)
+        o = default_opts()
+        o[A.OPTION_NITER] = niters
+        o[A.OPTION_TOLERANCE] = tol
+        o[A.OPTION_VERBOSITY] = verbosity
+        if stream is None:
+            s = torch.cuda.current_stream(dev).cuda_stream
+        else:
+            torch.cuda.current_stream(dev).synchronize()    # the buffers were filled there
+            s = stream
+        ptrs = (ptr_t * self.nmodes)(*[C.cast(C.c_void_p(b.data_ptr()), ptr_t) for b in bufs])
+        lam = np.zeros(rank)
+        fit = C.c_double()
+        its = C.c_int()
+        rc = getattr(self.lib, sym)(self.h, rank, ldm, _dptr(o), ptrs, _dptr(lam), C.byref(fit),
+                                    C.byref(its), C.c_void_p(s))
+        _check(rc, sym)
+        return fit.value, lam, [b[:, :rank] for b in bufs], its.value
+
     def shard(self, rank: int, count: int, device: int = -1) -> "Tensor":
         """Cut shard `rank` of `count` out of this (whole) tensor onto `device`
         (splatt_b200_tensor_shard): the equal-nnz chunk range of every stream, copied

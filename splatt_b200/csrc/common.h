@@ -101,6 +101,20 @@ struct splatt_b200_tensor {
   uint32_t * cta_done = nullptr;   // scratch of the in-kernel group barrier (lazily allocated)
 };
 
+// Run on the tensor's device, restore the caller's afterwards.
+struct DeviceGuard {
+  int prev = -1, want = -1;
+  bool ok = true;
+  explicit DeviceGuard(int dev) : want(dev) {
+    if (cudaGetDevice(&prev) != cudaSuccess) { ok = false; return; }
+    if (prev != want && cudaSetDevice(want) != cudaSuccess) {
+      fprintf(stderr, "SPLATT: cannot switch to CUDA device %d\n", want);
+      ok = false;
+    }
+  }
+  ~DeviceGuard() { if (ok && prev != want) cudaSetDevice(prev); }
+};
+
 // Kernel argument block (passed by value).
 struct MttkrpArgs {
   const SpRec *    rec;

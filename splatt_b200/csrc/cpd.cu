@@ -256,7 +256,9 @@ namespace {
 // ---------------------------------------------------------------------------
 
 // G(upper, row-major) += A^T A over a block of rows.  reference: mat_aTa src/matrix.c:414-455
-__global__ void k_gram(const double * __restrict__ A, unsigned long long I, int R, int lda,
+// T is the storage type of A (double or float); G and the arithmetic are fp64.
+template <class T>
+__global__ void k_gram(const T * __restrict__ A, unsigned long long I, int R, int lda,
                        double * __restrict__ G) {
   extern __shared__ double tile[];           // 32 rows x R
   const int nent = R * (R + 1) / 2;
@@ -273,7 +275,7 @@ __global__ void k_gram(const double * __restrict__ A, unsigned long long I, int 
        r0 += (unsigned long long)gridDim.x * 32) {
     const int rows = (int)min((unsigned long long)32, I - r0);
     for (int x = threadIdx.x; x < rows * R; x += blockDim.x)
-      tile[x] = A[(r0 + x / R) * lda + (x % R)];
+      tile[x] = static_cast<double>(A[(r0 + x / R) * lda + (x % R)]);
     __syncthreads();
     for (int t = 0; t < mine; ++t) {
       double a = acc[t];
@@ -377,7 +379,9 @@ __global__ void k_form_chol(const double * __restrict__ ata, int nmodes, int mod
 // One thread per row: X[i,:] = M1[i,:] * (L L^T)^-1 (or * P when info != 0).
 // reference: potrs call src/matrix.c:563 (nrhs = rows).  Row scratch lives in shared memory,
 // laid out [r][thread] so that accesses are conflict-free; L is read as a broadcast.
-__global__ void k_solve_rows(const double * __restrict__ M1, double * __restrict__ X,
+// Rows are stored as T and solved in fp64; the result is rounded to T once.
+template <class T>
+__global__ void k_solve_rows(const T * __restrict__ M1, T * __restrict__ X,
                              unsigned long long I, int R, int ld, const double * __restrict__ L,
                              const double * __restrict__ P, const int * __restrict__ info,
                              int only_fallback) {
@@ -391,28 +395,28 @@ __global__ void k_solve_rows(const double * __restrict__ M1, double * __restrict
   __syncthreads();
   const unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= I) return;
-  const int T = blockDim.x, t = threadIdx.x;
-  const double * row = M1 + i * ld;
-  for (int r = 0; r < R; ++r) xs[r * T + t] = row[r];
-  double * out = X + i * ld;
+  const int NT = blockDim.x, t = threadIdx.x;
+  const T * row = M1 + i * ld;
+  for (int r = 0; r < R; ++r) xs[r * NT + t] = static_cast<double>(row[r]);
+  T * out = X + i * ld;
   if (!use_p) {
     for (int p = 0; p < R; ++p) {           // L y = x
-      double s = xs[p * T + t];
-      for (int k = 0; k < p; ++k) s = fma(-Ls[k + p * R], xs[k * T + t], s);
-      xs[p * T + t] = s / Ls[p + p * R];
+      double s = xs[p * NT + t];
+      for (int k = 0; k < p; ++k) s = fma(-Ls[k + p * R], xs[k * NT + t], s);
+      xs[p * NT + t] = s / Ls[p + p * R];
     }
     for (int p = R - 1; p >= 0; --p) {      // L^T z = y
-      double s = xs[p * T + t];
-      for (int k = p + 1; k < R; ++k) s = fma(-Ls[p + k * R], xs[k * T + t], s);
+      double s = xs[p * NT + t];
+      for (int k = p + 1; k < R; ++k) s = fma(-Ls[p + k * R], xs[k * NT + t], s);
       s /= Ls[p + p * R];
-      xs[p * T + t] = s;
-      out[p] = s;
+      xs[p * NT + t] = s;
+      out[p] = static_cast<T>(s);
     }
   } else {
     for (int j = 0; j < R; ++j) {
       double s = 0;
-      for (int k = 0; k < R; ++k) s = fma(xs[k * T + t], Ls[j + k * R], s);
-      out[j] = s;
+      for (int k = 0; k < R; ++k) s = fma(xs[k * NT + t], Ls[j + k * R], s);
+      out[j] = static_cast<T>(s);
     }
   }
 }
@@ -427,9 +431,11 @@ __global__ void k_solve_rows(const double * __restrict__ M1, double * __restrict
 // X[i,:] = M1[i,:] * (L L^T)^-1, one thread per row, the row in registers, L (padded with an
 // identity block to RT) and its transpose in shared memory, read as 128-bit broadcasts.
 // reference: potrs call src/matrix.c:563.  (*info != 0: the generic kernel handles it.)
-template <int RT>
+// fp32 rows (ld % 4 == 0) move as float4; columns [R, RT) enter as 0 by selection, so the
+// unspecified pad columns of an fp32 M1 (NaN included) are loaded but never reach the solve.
+template <int RT, class T>
 __global__ void __launch_bounds__(128)
-k_solve_rows_reg(const double * __restrict__ M1, double * __restrict__ X, unsigned long long I,
+k_solve_rows_reg(const T * __restrict__ M1, T * __restrict__ X, unsigned long long I,
                  int R, int ld, const double * __restrict__ L, const int * __restrict__ info) {
   extern __shared__ __align__(16) double sm[];
   double * Ls  = sm;                    // RT*RT, row-major lower factor
@@ -450,11 +456,27 @@ k_solve_rows_reg(const double * __restrict__ M1, double * __restrict__ X, unsign
   const unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= I) return;
   double x[RT];
-  const double * row = M1 + i * ld;
+  const T * row = M1 + i * ld;
+  if constexpr (sizeof(T) == 8) {
 #pragma unroll
-  for (int r = 0; r < RT; r += 2) {
-    if (r + 1 < R) { const double2 v = *reinterpret_cast<const double2 *>(row + r); x[r] = v.x; x[r + 1] = v.y; }
-    else { x[r] = (r < R) ? row[r] : 0.0; x[r + 1] = 0.0; }
+    for (int r = 0; r < RT; r += 2) {
+      if (r + 1 < R) { const double2 v = *reinterpret_cast<const double2 *>(row + r); x[r] = v.x; x[r + 1] = v.y; }
+      else { x[r] = (r < R) ? row[r] : 0.0; x[r + 1] = 0.0; }
+    }
+  } else {
+    // (this shape keeps RT = 64 at 72 B of spill, under the fp64 instance's 88 B)
+#pragma unroll
+    for (int r = 0; r < RT; r += 4) {
+      if (r < R) {
+        const float4 v = *reinterpret_cast<const float4 *>(row + r);
+        x[r]     = v.x;
+        x[r + 1] = (r + 1 < R) ? (double)v.y : 0.0;
+        x[r + 2] = (r + 2 < R) ? (double)v.z : 0.0;
+        x[r + 3] = (r + 3 < R) ? (double)v.w : 0.0;
+      } else {
+        x[r] = x[r + 1] = x[r + 2] = x[r + 3] = 0.0;
+      }
+    }
   }
   // L y = x (forward), four independent partial sums per entry
 #pragma unroll
@@ -486,11 +508,24 @@ k_solve_rows_reg(const double * __restrict__ M1, double * __restrict__ X, unsign
     }
     x[p] = ((s0 + s1) + (s2 + s3)) * inv[p];
   }
-  double * out = X + i * ld;
+  T * out = X + i * ld;
+  if constexpr (sizeof(T) == 8) {
 #pragma unroll
-  for (int r = 0; r < RT; r += 2) {
-    if (r + 1 < R) *reinterpret_cast<double2 *>(out + r) = make_double2(x[r], x[r + 1]);
-    else if (r < R) out[r] = x[r];
+    for (int r = 0; r < RT; r += 2) {
+      if (r + 1 < R) *reinterpret_cast<double2 *>(out + r) = make_double2(x[r], x[r + 1]);
+      else if (r < R) out[r] = x[r];
+    }
+  } else {
+#pragma unroll
+    for (int r = 0; r < RT; r += 4) {
+      if (r + 3 < R) {
+        *reinterpret_cast<float4 *>(out + r) = make_float4((float)x[r], (float)x[r + 1],
+                                                           (float)x[r + 2], (float)x[r + 3]);
+      } else {
+#pragma unroll
+        for (int c = 0; c < 3; ++c) if (r + c < R) out[r + c] = (float)x[r + c];
+      }
+    }
   }
 }
 
@@ -498,9 +533,9 @@ k_solve_rows_reg(const double * __restrict__ M1, double * __restrict__ X, unsign
 // 64-row tiles of A through shared memory; two teams of threads (even / odd tile rows) each
 // hold the 4x4 blocks of the upper triangle of G in registers (one block per thread) and
 // flush them with one round of atomics per CTA.  reference: mat_aTa src/matrix.c:414-455
-template <int RT>
+template <int RT, class T>
 __global__ void __launch_bounds__(2 * ((RT / 4) * (RT / 4 + 1) / 2 + 31) / 32 * 32)
-k_gram_syrk(const double * __restrict__ A, unsigned long long I, int R, int lda,
+k_gram_syrk(const T * __restrict__ A, unsigned long long I, int R, int lda,
             double * __restrict__ G) {
   constexpr int NB     = RT / 4;                       // 4x4 blocks per side
   constexpr int NBLK   = NB * (NB + 1) / 2;            // blocks of the upper triangle
@@ -526,7 +561,7 @@ k_gram_syrk(const double * __restrict__ A, unsigned long long I, int R, int lda,
     const int rows = (int)min((unsigned long long)TR, I - r0);
     for (int x = threadIdx.x; x < TR * R; x += blockDim.x) {
       const int i = x / R, j = x % R;
-      tile[i * RT + j] = (i < rows) ? A[(r0 + i) * lda + j] : 0.0;
+      tile[i * RT + j] = (i < rows) ? static_cast<double>(A[(r0 + i) * lda + j]) : 0.0;
     }
     __syncthreads();
     if (active) {
@@ -559,7 +594,9 @@ k_gram_syrk(const double * __restrict__ A, unsigned long long I, int R, int lda,
 
 // Column sums of squares (two_norm) or column maxima of max(a, 0).
 // reference: p_mat_2norm src/matrix.c:86-144, p_mat_maxnorm :147-199
-__global__ void k_colnorm(const double * __restrict__ A, unsigned long long I, int R, int ld,
+// (fp32: held to the fp64 instance's 28 registers; left alone ptxas gives it 30)
+template <class T>
+__global__ void __maxnreg__(sizeof(T) == 4 ? 28 : 255) k_colnorm(const T * __restrict__ A, unsigned long long I, int R, int ld,
                           int two_norm, double * __restrict__ acc) {
   const int j = threadIdx.x % 32 + 32 * blockIdx.y;
   const int ty = threadIdx.x / 32, ny = blockDim.x / 32;
@@ -567,7 +604,7 @@ __global__ void k_colnorm(const double * __restrict__ A, unsigned long long I, i
   if (j < R)
     for (unsigned long long i = (unsigned long long)blockIdx.x * ny + ty; i < I;
          i += (unsigned long long)gridDim.x * ny) {
-      const double a = A[i * ld + j];
+      const double a = static_cast<double>(A[i * ld + j]);
       v = two_norm ? fma(a, a, v) : fmax(v, a);
     }
   __shared__ double red[8][33];
@@ -584,16 +621,19 @@ __global__ void k_finish_lambda(double * __restrict__ acc, int R, int two_norm,
   const int j = threadIdx.x + blockIdx.x * blockDim.x;
   if (j < R) lambda[j] = two_norm ? sqrt(acc[j]) : fmax(acc[j], 1.0);
 }
-__global__ void k_scale_cols(double * __restrict__ A, unsigned long long I, int R, int ld,
+// a /= lambda in fp64, rounded to T once
+template <class T>
+__global__ void k_scale_cols(T * __restrict__ A, unsigned long long I, int R, int ld,
                              const double * __restrict__ lambda) {
   const unsigned long long x = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (x >= I * R) return;
   const unsigned long long i = x / R;
   const int j = (int)(x % R);
-  A[i * ld + j] /= lambda[j];
+  A[i * ld + j] = static_cast<T>(static_cast<double>(A[i * ld + j]) / lambda[j]);
 }
 // inner += sum_i sum_r A[i,r] * M1[i,r] * lambda[r].  reference: p_tt_kruskal_inner src/cpd.c:171-218
-__global__ void k_inner(const double * __restrict__ A, const double * __restrict__ M1,
+template <class T>
+__global__ void k_inner(const T * __restrict__ A, const T * __restrict__ M1,
                         unsigned long long I, int R, int ld, const double * __restrict__ lambda,
                         double * __restrict__ inner) {
   double v = 0.0;
@@ -601,7 +641,7 @@ __global__ void k_inner(const double * __restrict__ A, const double * __restrict
        x += (unsigned long long)gridDim.x * blockDim.x) {
     const unsigned long long i = x / R;
     const int j = (int)(x % R);
-    v = fma(A[i * ld + j] * M1[i * ld + j], lambda[j], v);
+    v = fma(static_cast<double>(A[i * ld + j]) * static_cast<double>(M1[i * ld + j]), lambda[j], v);
   }
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
   __shared__ double red[32];
@@ -612,6 +652,33 @@ __global__ void k_inner(const double * __restrict__ A, const double * __restrict
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
     if (threadIdx.x == 0) atomicAdd(inner, v);
   }
+}
+
+// ||X||^2 as an fp64 sum of squares over one stream's record values: the device CPD entries
+// have no CSF to call csf_frobsq on.  reference: csf_frobsq src/csf.c:817-851
+__global__ void k_vals_sumsq(const SpRec * __restrict__ rec, unsigned long long n,
+                             double * __restrict__ out) {
+  double v = 0.0;
+  for (unsigned long long x = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; x < n;
+       x += (unsigned long long)gridDim.x * blockDim.x) {
+    const double a = rec[x].v;
+    v = fma(a, a, v);
+  }
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  __shared__ double red[32];
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+  __syncthreads();
+  if (threadIdx.x < 32) {
+    v = threadIdx.x < blockDim.x / 32 ? red[threadIdx.x] : 0.0;
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    if (threadIdx.x == 0) atomicAdd(out, v);
+  }
+}
+// post-processing (src/cpd.c:391-411): lambda_total *= the column 2-norms just divided out
+__global__ void k_fold_lambda(double * __restrict__ lambda_total, const double * __restrict__ norms,
+                              int R) {
+  const int j = threadIdx.x + blockIdx.x * blockDim.x;
+  if (j < R) lambda_total[j] *= norms[j];
 }
 
 // ---- pieces of the ROW-PARTITIONED tail (multi-GPU engine, multi.cu): every device works on
@@ -673,6 +740,25 @@ struct DevTail {
   int      rt = 0;                // R padded to 16 / 32 / 64: register-tiled solve + SYRK (0 = generic)
   bool     failed = false;        // a launch was rejected: results are not to be trusted
 
+  // shared-memory opt-in of the instances that serve storage type T
+  template <class T>
+  bool set_smem_attrs() {
+    bool ok = cudaFuncSetAttribute(k_solve_rows<T>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                   (R * R + R * solve_threads) * 8) == cudaSuccess &&
+              cudaFuncSetAttribute(k_gram<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, 32 * R * 8) == cudaSuccess;
+    if (ok && rt) {
+      const int sb = (2 * rt * rt + rt) * 8, gb = 64 * rt * 8;
+      cudaError_t e1 = cudaSuccess, e2 = cudaSuccess;
+      if (rt == 16) { e1 = cudaFuncSetAttribute(k_solve_rows_reg<16, T>, cudaFuncAttributeMaxDynamicSharedMemorySize, sb);
+                      e2 = cudaFuncSetAttribute(k_gram_syrk<16, T>, cudaFuncAttributeMaxDynamicSharedMemorySize, gb); }
+      if (rt == 32) { e1 = cudaFuncSetAttribute(k_solve_rows_reg<32, T>, cudaFuncAttributeMaxDynamicSharedMemorySize, sb);
+                      e2 = cudaFuncSetAttribute(k_gram_syrk<32, T>, cudaFuncAttributeMaxDynamicSharedMemorySize, gb); }
+      if (rt == 64) { e1 = cudaFuncSetAttribute(k_solve_rows_reg<64, T>, cudaFuncAttributeMaxDynamicSharedMemorySize, sb);
+                      e2 = cudaFuncSetAttribute(k_gram_syrk<64, T>, cudaFuncAttributeMaxDynamicSharedMemorySize, gb); }
+      if (e1 != cudaSuccess || e2 != cudaSuccess) { cudaGetLastError(); rt = 0; }
+    }
+    return ok;
+  }
   bool alloc(int N_, int R_, int ld_, cudaStream_t st) {
     N = N_; R = R_; ld = ld_; s = st;
     bool ok = cudaMalloc(&ata, sizeof(double) * N * R * R) == cudaSuccess &&
@@ -695,25 +781,12 @@ struct DevTail {
       cudaDeviceGetAttribute(&lim, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
       solve_threads = 128;
       while (solve_threads > 32 && (size_t)(R * R + R * solve_threads) * 8 > (size_t)lim) solve_threads /= 2;
-      ok = (size_t)(R * R + R * solve_threads) * 8 <= (size_t)lim && (size_t)R * R * 8 <= (size_t)lim &&
-           cudaFuncSetAttribute(k_form_chol, cudaFuncAttributeMaxDynamicSharedMemorySize, R * R * 8) == cudaSuccess &&
-           cudaFuncSetAttribute(k_solve_rows, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                (R * R + R * solve_threads) * 8) == cudaSuccess &&
-           cudaFuncSetAttribute(k_gram, cudaFuncAttributeMaxDynamicSharedMemorySize, 32 * R * 8) == cudaSuccess;
-      if (!ok) fprintf(stderr, "SPLATT: rank %d does not fit the device ALS tail (shared memory)\n", R);
       const char * ge = getenv("SPLATT_B200_TAIL_GENERIC");
       rt = (ge && atoi(ge) != 0) ? 0 : (R <= 16 ? 16 : (R <= 32 ? 32 : (R <= 64 ? 64 : 0)));
-      if (ok && rt) {
-        const int sb = (2 * rt * rt + rt) * 8, gb = 64 * rt * 8;
-        cudaError_t e1 = cudaSuccess, e2 = cudaSuccess;
-        if (rt == 16) { e1 = cudaFuncSetAttribute(k_solve_rows_reg<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, sb);
-                        e2 = cudaFuncSetAttribute(k_gram_syrk<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, gb); }
-        if (rt == 32) { e1 = cudaFuncSetAttribute(k_solve_rows_reg<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, sb);
-                        e2 = cudaFuncSetAttribute(k_gram_syrk<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, gb); }
-        if (rt == 64) { e1 = cudaFuncSetAttribute(k_solve_rows_reg<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, sb);
-                        e2 = cudaFuncSetAttribute(k_gram_syrk<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, gb); }
-        if (e1 != cudaSuccess || e2 != cudaSuccess) { cudaGetLastError(); rt = 0; }
-      }
+      ok = (size_t)(R * R + R * solve_threads) * 8 <= (size_t)lim && (size_t)R * R * 8 <= (size_t)lim &&
+           cudaFuncSetAttribute(k_form_chol, cudaFuncAttributeMaxDynamicSharedMemorySize, R * R * 8) == cudaSuccess &&
+           set_smem_attrs<double>() && set_smem_attrs<float>();
+      if (!ok) fprintf(stderr, "SPLATT: rank %d does not fit the device ALS tail (shared memory)\n", R);
     }
     return ok;
   }
@@ -729,65 +802,88 @@ struct DevTail {
     cudaFree(inner); cudaFree(info); cudaFree(jac_v); cudaFree(gpart);
     if (h_back) cudaFreeHost(h_back);
   }
-  void gram(const double * A, uint64_t I, int m) {
+  template <class T>
+  void gram(const T * A, uint64_t I, int m) {
     double * G = ata + (size_t)m * R * R;
     cudaMemsetAsync(G, 0, sizeof(double) * R * R, s);
     gram_into(A, I, G);
   }
   // G += A^T A (G is NOT zeroed here)
-  void gram_into(const double * A, uint64_t I, double * G) {
+  template <class T>
+  void gram_into(const T * A, uint64_t I, double * G) {
     if (I == 0) return;
     // the persistent SYRK pays one round of atomics per CTA: worth it from ~32 K rows on
     // (measured: 10 K x 32: 22.6 us vs 13.3 us generic; 1 M x 64: 0.74 ms vs 1.2 ms)
     if (rt && I >= 32768) {
       const unsigned blocks = (unsigned)std::min<uint64_t>((I + 63) / 64, 296);
       const size_t sm = (size_t)64 * rt * 8;
-      if (rt == 16) k_gram_syrk<16><<<blocks, 64, sm, s>>>(A, I, R, ld, G);
-      else if (rt == 32) k_gram_syrk<32><<<blocks, 128, sm, s>>>(A, I, R, ld, G);
-      else k_gram_syrk<64><<<blocks, 320, sm, s>>>(A, I, R, ld, G);
+      if (rt == 16) k_gram_syrk<16, T><<<blocks, 64, sm, s>>>(A, I, R, ld, G);
+      else if (rt == 32) k_gram_syrk<32, T><<<blocks, 128, sm, s>>>(A, I, R, ld, G);
+      else k_gram_syrk<64, T><<<blocks, 320, sm, s>>>(A, I, R, ld, G);
     } else {
       const unsigned blocks = (unsigned)std::min<uint64_t>((I + 31) / 32, 592);
-      k_gram<<<blocks, 256, 32 * R * 8, s>>>(A, I, R, ld, G);
+      k_gram<T><<<blocks, 256, 32 * R * 8, s>>>(A, I, R, ld, G);
     }
     check("k_gram");
     spb200_count_launches(1);
   }
   // one mode step after the MTTKRP: d_out (M1) -> d_mat (new factor), lambda, Gram
-  void mode_step(const double * d_out, double * d_mat, uint64_t I, int m, bool two_norm) {
+  template <class T>
+  void mode_step(const T * d_out, T * d_mat, uint64_t I, int m, bool two_norm) {
     solve(d_out, d_mat, I, m);
     cudaMemsetAsync(lam_acc, 0, sizeof(double) * R, s);
     dim3 g((unsigned)std::min<uint64_t>((I + 7) / 8, 1184), (R + 31) / 32);
-    k_colnorm<<<g, 256, 0, s>>>(d_mat, I, R, ld, two_norm ? 1 : 0, lam_acc);
+    k_colnorm<T><<<g, 256, 0, s>>>(d_mat, I, R, ld, two_norm ? 1 : 0, lam_acc);
     k_finish_lambda<<<(R + 127) / 128, 128, 0, s>>>(lam_acc, R, two_norm ? 1 : 0, lambda);
-    k_scale_cols<<<(unsigned)((I * R + 255) / 256), 256, 0, s>>>(d_mat, I, R, ld, lambda);
+    k_scale_cols<T><<<(unsigned)((I * R + 255) / 256), 256, 0, s>>>(d_mat, I, R, ld, lambda);
     check("normalise");
     spb200_count_launches(3);
     gram(d_mat, I, m);
   }
   // normal matrix of mode m + Cholesky, then the row solves of `I` rows
-  void solve(const double * d_out, double * d_mat, uint64_t I, int m) {
+  template <class T>
+  void solve(const T * d_out, T * d_mat, uint64_t I, int m) {
     k_form_chol<<<1, 256, R * R * 8, s>>>(ata, N, m, R, chol, pinv, jac_v, info);
     check("k_form_chol");
     spb200_count_launches(1);
     if (I == 0) return;
-    const int T = solve_threads;
+    const int NT = solve_threads;
     if (rt) {
       // register-tiled solve when the Cholesky succeeded (it returns at once otherwise) ...
       const size_t sm = (size_t)(2 * rt * rt + rt) * 8;
       const unsigned nb = (unsigned)((I + 127) / 128);
-      if (rt == 16) k_solve_rows_reg<16><<<nb, 128, sm, s>>>(d_out, d_mat, I, R, ld, chol, info);
-      else if (rt == 32) k_solve_rows_reg<32><<<nb, 128, sm, s>>>(d_out, d_mat, I, R, ld, chol, info);
-      else k_solve_rows_reg<64><<<nb, 128, sm, s>>>(d_out, d_mat, I, R, ld, chol, info);
+      if (rt == 16) k_solve_rows_reg<16, T><<<nb, 128, sm, s>>>(d_out, d_mat, I, R, ld, chol, info);
+      else if (rt == 32) k_solve_rows_reg<32, T><<<nb, 128, sm, s>>>(d_out, d_mat, I, R, ld, chol, info);
+      else k_solve_rows_reg<64, T><<<nb, 128, sm, s>>>(d_out, d_mat, I, R, ld, chol, info);
       // ... and the generic kernel only for the pseudo-inverse fallback (info != 0)
-      k_solve_rows<<<(unsigned)((I + T - 1) / T), T, (R * R + R * T) * 8, s>>>(
+      k_solve_rows<T><<<(unsigned)((I + NT - 1) / NT), NT, (R * R + R * NT) * 8, s>>>(
           d_out, d_mat, I, R, ld, chol, pinv, info, 1);
       spb200_count_launches(1);
     } else {
-      k_solve_rows<<<(unsigned)((I + T - 1) / T), T, (R * R + R * T) * 8, s>>>(
+      k_solve_rows<T><<<(unsigned)((I + NT - 1) / NT), NT, (R * R + R * NT) * 8, s>>>(
           d_out, d_mat, I, R, ld, chol, pinv, info, 0);
     }
     check("k_solve_rows");
     spb200_count_launches(1);
+  }
+
+  // post-processing on the device (src/cpd.c:391-411): 2-normalise every factor, folding the
+  // norms into lambda_total (R doubles, device; holds the ALS lambda on entry)
+  template <class T>
+  void postprocess(T * const * d_mats, const uint64_t * dims, double * lambda_total) {
+    for (int m = 0; m < N; ++m) {
+      const uint64_t I = dims[m];
+      cudaMemsetAsync(lam_acc, 0, sizeof(double) * R, s);
+      if (I) {
+        dim3 g((unsigned)std::min<uint64_t>((I + 7) / 8, 1184), (R + 31) / 32);
+        k_colnorm<T><<<g, 256, 0, s>>>(d_mats[m], I, R, ld, 1, lam_acc);
+      }
+      k_finish_lambda<<<(R + 127) / 128, 128, 0, s>>>(lam_acc, R, 1, lambda);
+      if (I) k_scale_cols<T><<<(unsigned)((I * R + 255) / 256), 256, 0, s>>>(d_mats[m], I, R, ld, lambda);
+      k_fold_lambda<<<(R + 127) / 128, 128, 0, s>>>(lambda_total, lambda, R);
+      check("post-process");
+      spb200_count_launches(I ? 4 : 2);
+    }
   }
 
   // ---- row-partitioned tail (see the kernels above)
@@ -796,7 +892,7 @@ struct DevTail {
     solve(m1, x, rows, m);
     if (rows) {
       dim3 g((unsigned)std::min<uint64_t>((rows + 7) / 8, 1184), (R + 31) / 32);
-      k_colnorm<<<g, 256, 0, s>>>(x, rows, R, ld, two_norm ? 1 : 0, lam_acc);
+      k_colnorm<double><<<g, 256, 0, s>>>(x, rows, R, ld, two_norm ? 1 : 0, lam_acc);
     }
     k_publish_zero<<<1, 128, 0, s>>>(lam_acc, mc_norm_slot, R);
     check("norm partial");
@@ -825,6 +921,151 @@ struct DevTail {
     spb200_count_launches(1);
   }
 };
+
+// fit = 1 - ||X - K|| / ||X||  (reference: p_calc_fit src/cpd.c:237-265)
+double cpd_fit(const std::vector<std::vector<double>> & ata, const double * lambda, int N, int R,
+               double ttnormsq, double inner) {
+  const double norm_mats = kruskal_norm(ata, lambda, N, R);
+  double residual = ttnormsq + norm_mats - 2 * inner;
+  if (residual > 0.) residual = std::sqrt(residual);
+  return 1 - residual / std::sqrt(ttnormsq);
+}
+
+int mttkrp_t(const splatt_b200_tensor * t, int m, int R, int ldm, double * const * d_mats,
+             double * d_out, cudaStream_t s) {
+  return splatt_b200_mttkrp(t, m, R, ldm, d_mats, d_out, s);
+}
+int mttkrp_t(const splatt_b200_tensor * t, int m, int R, int ldm, float * const * d_mats,
+             float * d_out, cudaStream_t s) {
+  return splatt_b200_mttkrp_f32(t, m, R, ldm, d_mats, d_out, s);
+}
+
+// CPD-ALS with the dense tail on the device (reference: cpd_als_iterate src/cpd.c:318-373):
+// per mode MTTKRP -> tail.mode_step; per iteration one small read-back (Grams, lambda, inner
+// product, solver info) for the fit -- the loop's only host synchronisation.  d_mats hold the
+// start on entry (their Grams are formed here) and the factors of the last iteration on return,
+// not post-processed.  d_out: M1 scratch of max(dims) x ldm.  lambda: R host doubles, the last
+// iteration's.  false when a launch failed.
+template <class T>
+bool run_device_als(const splatt_b200_tensor * t, T * const * d_mats, T * d_out, int ldm,
+                    DevTail & tail, double ttnormsq, const double * options, double * lambda,
+                    double * fit_out, uint64_t * iterations_out) {
+  const int N = tail.N, R = tail.R;
+  const uint64_t * dims = t->dims;
+  const cudaStream_t stream = tail.s;
+  const int verbosity = (int)options[SPLATT_OPTION_VERBOSITY];
+  const uint64_t niters = (uint64_t)options[SPLATT_OPTION_NITER];
+  std::vector<std::vector<double>> ata(N, std::vector<double>((size_t)R * R));
+  double fit = 0, oldfit = 0;
+  uint64_t its = 0;
+  bool ok = true;
+  for (int m = 0; m < N; ++m) tail.gram(d_mats[m], dims[m], m);
+  const size_t nb = (size_t)N * R * R;
+  for (uint64_t it = 0; it < niters && ok; ++it) {
+    auto t0 = std::chrono::steady_clock::now();
+    for (int m = 0; m < N && ok; ++m) {
+      if (mttkrp_t(t, m, R, ldm, d_mats, d_out, stream) != SPLATT_SUCCESS) { ok = false; break; }
+      tail.mode_step(d_out, d_mats[m], dims[m], m, it == 0);
+    }
+    if (!ok) break;
+    cudaMemsetAsync(tail.inner, 0, sizeof(double), stream);
+    k_inner<T><<<296, 256, 0, stream>>>(d_mats[N - 1], d_out, dims[N - 1], R, ldm, tail.lambda,
+                                        tail.inner);
+    spb200_count_launches(1);
+    cudaMemcpyAsync(tail.h_back, tail.ata, nb * 8, cudaMemcpyDeviceToHost, stream);
+    cudaMemcpyAsync(tail.h_back + nb, tail.lambda, R * 8, cudaMemcpyDeviceToHost, stream);
+    cudaMemcpyAsync(tail.h_back + nb + R, tail.inner, 8, cudaMemcpyDeviceToHost, stream);
+    cudaMemcpyAsync(tail.h_back + nb + R + 1, tail.info, 4, cudaMemcpyDeviceToHost, stream);
+    if (cudaStreamSynchronize(stream) != cudaSuccess || tail.failed) { ok = false; break; }
+    for (int m = 0; m < N; ++m)
+      memcpy(ata[m].data(), tail.h_back + (size_t)m * R * R, sizeof(double) * R * R);
+    memcpy(lambda, tail.h_back + nb, sizeof(double) * R);
+    int info_last = 0;
+    memcpy(&info_last, tail.h_back + nb + R + 1, sizeof(int));
+    if (info_last)
+      fprintf(stderr, "SPLATT: Gram matrix is not SPD. Used pseudo-inverse.\n");
+    fit = cpd_fit(ata, lambda, N, R, ttnormsq, tail.h_back[nb + R]);
+    its = it + 1;
+    if (verbosity > SPLATT_VERBOSITY_NONE)
+      printf("  its = %3llu (%0.3fs)  fit = %0.5f  delta = %+0.4e\n", (unsigned long long)it + 1,
+             std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count(), fit,
+             fit - oldfit);
+    if (fit == 1. || (it > 0 && std::fabs(fit - oldfit) < options[SPLATT_OPTION_TOLERANCE]))
+      break;
+    oldfit = fit;
+  }
+  *fit_out = fit;
+  *iterations_out = its;
+  return ok;
+}
+
+// splatt_b200_cpd_als_device / _f32: CPD-ALS of a device tensor from device factors.
+template <class T>
+int cpd_als_device(const char * name, const splatt_b200_tensor * t, int R, int ldm,
+                   const double * options, T * const * d_factors, double * lambda_out,
+                   double * fit_out, int * iterations_out, void * stream) {
+  constexpr int align = sizeof(T) == 4 ? 4 : 2;     // row alignment of the MTTKRP
+  bool bad = !t || !options || !d_factors || R < 1 || R > 128 || ldm % align != 0 ||
+             ldm < (R + align - 1) / align * align;
+  bad = bad || t->nmodes < 2 || t->nmodes > SPB200_MAXN || t->shard_count > 1 || t->streams.empty();
+  for (int m = 0; !bad && m < t->nmodes; ++m)
+    bad = !d_factors[m] || reinterpret_cast<uintptr_t>(d_factors[m]) % 16 != 0;
+  if (bad) {
+    fprintf(stderr, "SPLATT: %s: bad arguments\n", name);
+    return SPLATT_ERROR_BADINPUT;
+  }
+  DeviceGuard g(t->device);
+  if (!g.ok) return SPLATT_ERROR_BADINPUT;
+  const int N = t->nmodes;
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  uint64_t maxdim = 0;
+  for (int m = 0; m < N; ++m) maxdim = std::max(maxdim, t->dims[m]);
+  T * d_out = nullptr;
+  double * d_lambda = nullptr;
+  DevTail tail;
+  bool alloc_ok = cudaMalloc(&d_out, std::max<uint64_t>(maxdim, 1) * (size_t)ldm * sizeof(T)) == cudaSuccess &&
+                  cudaMalloc(&d_lambda, sizeof(double) * R) == cudaSuccess &&
+                  tail.alloc(N, R, ldm, s);
+  bool ok = alloc_ok;
+  double ttnormsq = 0, fit = 0;
+  uint64_t its = 0;
+  std::vector<double> lambda(R);
+  if (ok) {
+    const FiberStream & fs = t->streams[0];
+    cudaMemsetAsync(tail.inner, 0, sizeof(double), s);
+    if (fs.nrec) {
+      k_vals_sumsq<<<(unsigned)std::min<uint64_t>((fs.nrec + 255) / 256, 1184), 256, 0, s>>>(
+          fs.rec, fs.nrec, tail.inner);
+      tail.check("k_vals_sumsq");
+      spb200_count_launches(1);
+    }
+    ok = cudaMemcpyAsync(tail.h_back, tail.inner, 8, cudaMemcpyDeviceToHost, s) == cudaSuccess &&
+         cudaStreamSynchronize(s) == cudaSuccess && !tail.failed;
+    ttnormsq = tail.h_back[0];
+  }
+  ok = ok && run_device_als<T>(t, d_factors, d_out, ldm, tail, ttnormsq, options, lambda.data(),
+                               &fit, &its);
+  if (ok) {
+    ok = cudaMemcpyAsync(d_lambda, lambda.data(), sizeof(double) * R, cudaMemcpyHostToDevice, s) == cudaSuccess;
+    tail.postprocess(d_factors, t->dims, d_lambda);
+    ok = ok && cudaMemcpyAsync(tail.h_back, d_lambda, sizeof(double) * R, cudaMemcpyDeviceToHost, s) == cudaSuccess &&
+         cudaStreamSynchronize(s) == cudaSuccess && !tail.failed;
+  }
+  if (ok) {
+    if (lambda_out) memcpy(lambda_out, tail.h_back, sizeof(double) * R);
+    if (fit_out) *fit_out = fit;
+    if (iterations_out) *iterations_out = (int)its;
+  }
+  cudaStreamSynchronize(s);
+  cudaFree(d_out);
+  cudaFree(d_lambda);
+  tail.release();
+  if (!ok) {
+    fprintf(stderr, "SPLATT: %s failed (%s)\n", name, cudaGetErrorString(cudaGetLastError()));
+    return alloc_ok ? SPLATT_ERROR_BADINPUT : SPLATT_ERROR_NOMEMORY;
+  }
+  return SPLATT_SUCCESS;
+}
 
 }  // namespace
 
@@ -919,12 +1160,7 @@ int splatt_cpd_als(splatt_csf const * const tensors, splatt_idx_t const nfactors
       printf("  its = %3llu (%0.3fs)  fit = %0.5f  delta = %+0.4e\n", (unsigned long long)it + 1,
              secs, fit, fit - oldfit);
   };
-  auto fit_from = [&](double inner) {     // src/cpd.c:237-265
-    const double norm_mats = kruskal_norm(ata, lambda, N, R);
-    double residual = ttnormsq + norm_mats - 2 * inner;
-    if (residual > 0.) residual = std::sqrt(residual);
-    fit = 1 - residual / std::sqrt(ttnormsq);
-  };
+  auto fit_from = [&](double inner) { fit = cpd_fit(ata, lambda, N, R, ttnormsq, inner); };
 
   if (ok && host_tail) {
     for (int m = 0; m < N; ++m) gram(mats[m], dims[m], R, ata[m].data());
@@ -960,38 +1196,8 @@ int splatt_cpd_als(splatt_csf const * const tensors, splatt_idx_t const nfactors
     }
   } else if (ok) {
     // ---- everything on the device; one small read-back per iteration for the fit
-    for (int m = 0; m < N; ++m) tail.gram(d_mats[m], dims[m], m);
-    const size_t nb = (size_t)N * R * R;
-    for (uint64_t it = 0; it < niters && ok; ++it) {
-      auto t0 = std::chrono::steady_clock::now();
-      for (int m = 0; m < N && ok; ++m) {
-        rc = splatt_b200_mttkrp(T, m, R, ldm, d_mats, d_out, stream);
-        if (rc != SPLATT_SUCCESS) { ok = false; break; }
-        tail.mode_step(d_out, d_mats[m], dims[m], m, it == 0);
-      }
-      if (!ok) break;
-      cudaMemsetAsync(tail.inner, 0, sizeof(double), stream);
-      k_inner<<<296, 256, 0, stream>>>(d_mats[N - 1], d_out, dims[N - 1], R, ldm, tail.lambda,
-                                       tail.inner);
-      spb200_count_launches(1);
-      cudaMemcpyAsync(tail.h_back, tail.ata, nb * 8, cudaMemcpyDeviceToHost, stream);
-      cudaMemcpyAsync(tail.h_back + nb, tail.lambda, R * 8, cudaMemcpyDeviceToHost, stream);
-      cudaMemcpyAsync(tail.h_back + nb + R, tail.inner, 8, cudaMemcpyDeviceToHost, stream);
-      cudaMemcpyAsync(tail.h_back + nb + R + 1, tail.info, 4, cudaMemcpyDeviceToHost, stream);
-      if (cudaStreamSynchronize(stream) != cudaSuccess || tail.failed) { ok = false; break; }
-      for (int m = 0; m < N; ++m)
-        memcpy(ata[m].data(), tail.h_back + (size_t)m * R * R, sizeof(double) * R * R);
-      memcpy(lambda, tail.h_back + nb, sizeof(double) * R);
-      int info_last = 0;
-      memcpy(&info_last, tail.h_back + nb + R + 1, sizeof(int));
-      if (info_last)
-        fprintf(stderr, "SPLATT: Gram matrix is not SPD. Used pseudo-inverse.\n");
-      fit_from(tail.h_back[nb + R]);
-      report(it, std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count());
-      if (fit == 1. || (it > 0 && std::fabs(fit - oldfit) < options[SPLATT_OPTION_TOLERANCE]))
-        break;
-      oldfit = fit;
-    }
+    uint64_t its = 0;
+    ok = run_device_als<double>(T, d_mats, d_out, ldm, tail, ttnormsq, options, lambda, &fit, &its);
     for (int m = 0; m < N && ok; ++m) ok = d2h(mats[m], d_mats[m], dims[m]) == cudaSuccess;
     ok = ok && cudaStreamSynchronize(stream) == cudaSuccess;
   }
@@ -1027,6 +1233,43 @@ int splatt_cpd_als(splatt_csf const * const tensors, splatt_idx_t const nfactors
 // with the same kernels splatt_cpd_als uses (splatt_b200/parallel.py:cpd_als_sharded).
 // ---------------------------------------------------------------------------
 struct splatt_b200_als_tail { DevTail t; };
+
+}  // extern "C"
+
+namespace {
+
+template <class T>
+int tail_fit(splatt_b200_als_tail * h, const T * d_last_factor, const T * d_last_m1, uint64_t rows,
+             double ttnormsq, double * fit_out, double * lambda_out) {
+  if (!h || !fit_out) return SPLATT_ERROR_BADINPUT;
+  DevTail & t = h->t;
+  const int N = t.N, R = t.R;
+  const size_t nb = (size_t)N * R * R;
+  cudaMemsetAsync(t.inner, 0, sizeof(double), t.s);
+  k_inner<T><<<296, 256, 0, t.s>>>(d_last_factor, d_last_m1, rows, R, t.ld, t.lambda, t.inner);
+  spb200_count_launches(1);
+  cudaMemcpyAsync(t.h_back, t.ata, nb * 8, cudaMemcpyDeviceToHost, t.s);
+  cudaMemcpyAsync(t.h_back + nb, t.lambda, R * 8, cudaMemcpyDeviceToHost, t.s);
+  cudaMemcpyAsync(t.h_back + nb + R, t.inner, 8, cudaMemcpyDeviceToHost, t.s);
+  if (cudaStreamSynchronize(t.s) != cudaSuccess || t.failed) return SPLATT_ERROR_BADINPUT;
+  std::vector<std::vector<double>> ata(N, std::vector<double>((size_t)R * R));
+  for (int m = 0; m < N; ++m)
+    memcpy(ata[m].data(), t.h_back + (size_t)m * R * R, sizeof(double) * R * R);
+  const double * lambda = t.h_back + nb;
+  *fit_out = cpd_fit(ata, lambda, N, R, ttnormsq, t.h_back[nb + R]);
+  if (lambda_out) memcpy(lambda_out, lambda, sizeof(double) * R);
+  return SPLATT_SUCCESS;
+}
+
+// the fp32 tail entries need 16-byte rows (ldm % 4 == 0) and 16-byte aligned matrices
+bool f32_tail_ok(const splatt_b200_als_tail * h, const float * a, const float * b) {
+  return h && h->t.ld % 4 == 0 && a && b && reinterpret_cast<uintptr_t>(a) % 16 == 0 &&
+         reinterpret_cast<uintptr_t>(b) % 16 == 0;
+}
+
+}  // namespace
+
+extern "C" {
 
 int splatt_b200_als_tail_create(int nmodes, int ncolumns, int ldm, void * stream,
                                 splatt_b200_als_tail ** out) {
@@ -1069,27 +1312,44 @@ int splatt_b200_als_tail_update(splatt_b200_als_tail * h, int mode, double const
 int splatt_b200_als_tail_fit(splatt_b200_als_tail * h, double const * d_last_factor,
                              double const * d_last_m1, uint64_t rows, double ttnormsq,
                              double * fit_out, double * lambda_out) {
-  if (!h || !fit_out) return SPLATT_ERROR_BADINPUT;
-  DevTail & t = h->t;
-  const int N = t.N, R = t.R;
-  const size_t nb = (size_t)N * R * R;
-  cudaMemsetAsync(t.inner, 0, sizeof(double), t.s);
-  k_inner<<<296, 256, 0, t.s>>>(d_last_factor, d_last_m1, rows, R, t.ld, t.lambda, t.inner);
-  spb200_count_launches(1);
-  cudaMemcpyAsync(t.h_back, t.ata, nb * 8, cudaMemcpyDeviceToHost, t.s);
-  cudaMemcpyAsync(t.h_back + nb, t.lambda, R * 8, cudaMemcpyDeviceToHost, t.s);
-  cudaMemcpyAsync(t.h_back + nb + R, t.inner, 8, cudaMemcpyDeviceToHost, t.s);
-  if (cudaStreamSynchronize(t.s) != cudaSuccess || t.failed) return SPLATT_ERROR_BADINPUT;
-  std::vector<std::vector<double>> ata(N, std::vector<double>((size_t)R * R));
-  for (int m = 0; m < N; ++m)
-    memcpy(ata[m].data(), t.h_back + (size_t)m * R * R, sizeof(double) * R * R);
-  const double * lambda = t.h_back + nb;
-  const double norm_mats = kruskal_norm(ata, lambda, N, R);
-  double residual = ttnormsq + norm_mats - 2 * t.h_back[nb + R];
-  if (residual > 0.) residual = std::sqrt(residual);
-  *fit_out = 1 - residual / std::sqrt(ttnormsq);
-  if (lambda_out) memcpy(lambda_out, lambda, sizeof(double) * R);
-  return SPLATT_SUCCESS;
+  return tail_fit(h, d_last_factor, d_last_m1, rows, ttnormsq, fit_out, lambda_out);
+}
+
+int splatt_b200_als_tail_gram_f32(splatt_b200_als_tail * h, int mode, float const * d_factor,
+                                  uint64_t rows) {
+  if (!f32_tail_ok(h, d_factor, d_factor) || mode < 0 || mode >= h->t.N) return SPLATT_ERROR_BADINPUT;
+  h->t.gram(d_factor, rows, mode);
+  return (cudaGetLastError() == cudaSuccess && !h->t.failed) ? SPLATT_SUCCESS : SPLATT_ERROR_BADINPUT;
+}
+
+int splatt_b200_als_tail_update_f32(splatt_b200_als_tail * h, int mode, float const * d_m1,
+                                    float * d_factor, uint64_t rows, int first_iteration) {
+  if (!f32_tail_ok(h, d_m1, d_factor) || mode < 0 || mode >= h->t.N) return SPLATT_ERROR_BADINPUT;
+  h->t.mode_step(d_m1, d_factor, rows, mode, first_iteration != 0);
+  return (cudaGetLastError() == cudaSuccess && !h->t.failed) ? SPLATT_SUCCESS : SPLATT_ERROR_BADINPUT;
+}
+
+int splatt_b200_als_tail_fit_f32(splatt_b200_als_tail * h, float const * d_last_factor,
+                                 float const * d_last_m1, uint64_t rows, double ttnormsq,
+                                 double * fit_out, double * lambda_out) {
+  if (!f32_tail_ok(h, d_last_factor, d_last_m1)) return SPLATT_ERROR_BADINPUT;
+  return tail_fit(h, d_last_factor, d_last_m1, rows, ttnormsq, fit_out, lambda_out);
+}
+
+int splatt_b200_cpd_als_device(splatt_b200_tensor const * t, int ncolumns, int ldm,
+                               double const * options, double * const * d_factors,
+                               double * lambda_out, double * fit_out, int * iterations_out,
+                               void * stream) {
+  return cpd_als_device("splatt_b200_cpd_als_device", t, ncolumns, ldm, options, d_factors,
+                        lambda_out, fit_out, iterations_out, stream);
+}
+
+int splatt_b200_cpd_als_device_f32(splatt_b200_tensor const * t, int ncolumns, int ldm,
+                                   double const * options, float * const * d_factors,
+                                   double * lambda_out, double * fit_out, int * iterations_out,
+                                   void * stream) {
+  return cpd_als_device("splatt_b200_cpd_als_device_f32", t, ncolumns, ldm, options, d_factors,
+                        lambda_out, fit_out, iterations_out, stream);
 }
 
 }  // extern "C"

@@ -68,20 +68,6 @@ void spb200_shard_chunks(uint64_t nnz, int rank, int nshards, uint64_t * c0, uin
 
 namespace {
 
-// Run on the tensor's device, restore the caller's afterwards.
-struct DeviceGuard {
-  int prev = -1, want = -1;
-  bool ok = true;
-  explicit DeviceGuard(int dev) : want(dev) {
-    if (cudaGetDevice(&prev) != cudaSuccess) { ok = false; return; }
-    if (prev != want && cudaSetDevice(want) != cudaSuccess) {
-      fprintf(stderr, "SPLATT: cannot switch to CUDA device %d\n", want);
-      ok = false;
-    }
-  }
-  ~DeviceGuard() { if (ok && prev != want) cudaSetDevice(prev); }
-};
-
 struct DevCoo {
   int N = 0;
   uint64_t nnz = 0;
