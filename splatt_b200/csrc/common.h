@@ -27,6 +27,7 @@
 // Everything a traversal needs arrives as three perfectly sequential streams
 // (rec, up[*], desc); the only random accesses are the factor-row gathers.
 #pragma once
+#include <chrono>
 #include <cstdint>
 #include <cstddef>
 #include <cstdio>
@@ -212,6 +213,51 @@ int spb200_launch_tiled_root3(const FiberStream & s, int ldm, int col_begin, int
                               cudaStream_t stream);
 // rows of a leaf tile that fit the kernel's smem beside an accumulator of acc_rows rows
 uint32_t spb200_tiled_rows_for(uint32_t acc_rows);
+
+// Copy a host row-major I x J matrix into a device I x ldm buffer, and back.
+inline cudaError_t h2d_matrix(double * dst, int ldm, const double * src, uint64_t I, uint64_t J,
+                              cudaStream_t s) {
+  if ((uint64_t)ldm == J) return cudaMemcpyAsync(dst, src, I * J * 8, cudaMemcpyHostToDevice, s);
+  return cudaMemcpy2DAsync(dst, (size_t)ldm * 8, src, J * 8, J * 8, I, cudaMemcpyHostToDevice, s);
+}
+inline cudaError_t d2h_matrix(double * dst, const double * src, int ldm, uint64_t I, uint64_t J,
+                              cudaStream_t s) {
+  if ((uint64_t)ldm == J) return cudaMemcpyAsync(dst, src, I * J * 8, cudaMemcpyDeviceToHost, s);
+  return cudaMemcpy2DAsync(dst, J * 8, src, (size_t)ldm * 8, J * 8, I, cudaMemcpyDeviceToHost, s);
+}
+
+// cpd.cu -- what the CPD-ALS drivers (cpd.cu, multi.cu) share ----------------------------------
+// Iteration control of ALS (reference: cpd_als_iterate src/cpd.c:356-373): start() when an
+// iteration begins; done(it, fit) when its fit is known prints the "its" line (verbosity above
+// NONE) and returns whether the loop stops there.
+struct AlsIterations {
+  uint64_t niters;
+  double   tol;
+  int      verbosity;
+  double   oldfit = 0;
+  std::chrono::steady_clock::time_point t0;
+  explicit AlsIterations(const double * options);
+  void start();
+  bool done(uint64_t it, double fit);
+};
+
+// The host side of a splatt_kruskal result: factors and lambda from the reference's random start
+// (src/cpd.c:36-40) to the post-processed result (src/cpd.c:391-411).
+struct HostKruskal {
+  int N = 0, R = 0;
+  uint64_t dims[SPB200_MAXN] = {0};
+  double * mats[SPB200_MAXN] = {nullptr};   // dims[m] x R, row-major
+  double * lambda = nullptr;
+  HostKruskal() = default;
+  HostKruskal(const HostKruskal &) = delete;
+  ~HostKruskal();                           // frees what finish() has not handed over
+  // allocate the factors and lambda and draw the start; false when out of memory
+  bool start(int N, const uint64_t * dims, int R);
+  // 2-normalise every factor into lambda and hand the result over to `out`
+  void finish(double fit, splatt_kruskal * out);
+};
+
+double spb200_csf_frobsq(const splatt_csf * t);   // ||X||^2 (reference: src/csf.c:817-851)
 
 // cpd.cu -- row-partitioned ALS tail steps (multi-GPU engine).  Every device works on its own
 // row slice; partial column norms / Grams go to per-device slots of the multicast region and

@@ -15,6 +15,7 @@
 #include <cmath>
 #include <cstdlib>
 #include <cstring>
+#include <type_traits>
 #include <vector>
 
 namespace {
@@ -52,13 +53,13 @@ void gram(const double * A, uint64_t I, int R, double * G) {
 // NOTE: in the reference the `1 + reg` written on the diagonal is immediately
 // overwritten by the row fill (src/matrix.c:45-51), i.e. the regularisation
 // parameter has no effect; that effective behaviour is reproduced.
-void form_normal_matrix(const std::vector<std::vector<double>> & ata, int mode, int N, int R,
-                        double * neq) {
+// ata: the N Grams, R x R each, one after the other
+void form_normal_matrix(const double * ata, int mode, int N, int R, double * neq) {
   for (int x = 0; x < R * R; ++x) neq[x] = 1.0;
   for (int m = 0; m < N; ++m) {
     if (m == mode) continue;
     for (int i = 0; i < R; ++i)
-      for (int j = i; j < R; ++j) neq[j + i * R] *= ata[m][j + i * R];
+      for (int j = i; j < R; ++j) neq[j + i * R] *= ata[(size_t)m * R * R + j + i * R];
   }
   for (int i = 0; i < R; ++i)
     for (int j = 0; j < i; ++j) neq[j + i * R] = neq[i + j * R];
@@ -99,11 +100,11 @@ void cholesky_solve_rows(const double * L, int R, double * X, uint64_t I) {
   }
 }
 
-// Minimum-norm least squares for a symmetric (possibly singular) G: the role of
-// the reference's GELSS fallback (src/matrix.c:566-603).  Jacobi eigen-solve,
-// pseudo-inverse with the LAPACK default cut-off (rcond < 0 -> machine eps).
-void pinv_solve_rows(const double * Gin, int R, double * X, uint64_t I) {
-  std::vector<double> A(Gin, Gin + (size_t)R * R), V((size_t)R * R, 0.0);
+// Pseudo-inverse P of the symmetric R x R matrix A (overwritten) by a Jacobi eigen-solve, with
+// the LAPACK default cut-off (rcond < 0 -> machine eps); V: R x R scratch.  Returns the
+// effective rank.  Runs on the host (pinv_solve_rows) and in one thread of k_form_chol.
+__host__ __device__ int jacobi_pinv(double * A, double * V, int R, double * P) {
+  for (int x = 0; x < R * R; ++x) V[x] = 0.0;
   for (int i = 0; i < R; ++i) V[i + i * R] = 1.0;
   for (int sweep = 0; sweep < 64; ++sweep) {
     double off = 0;
@@ -113,10 +114,10 @@ void pinv_solve_rows(const double * Gin, int R, double * X, uint64_t I) {
     for (int p = 0; p < R; ++p)
       for (int q = p + 1; q < R; ++q) {
         const double apq = A[q + p * R];
-        if (std::fabs(apq) < 1e-300) continue;
+        if (fabs(apq) < 1e-300) continue;
         const double theta = (A[q + q * R] - A[p + p * R]) / (2.0 * apq);
-        const double t = (theta >= 0 ? 1.0 : -1.0) / (std::fabs(theta) + std::sqrt(theta * theta + 1.0));
-        const double c = 1.0 / std::sqrt(t * t + 1.0), s = t * c;
+        const double t = (theta >= 0 ? 1.0 : -1.0) / (fabs(theta) + sqrt(theta * theta + 1.0));
+        const double c = 1.0 / sqrt(t * t + 1.0), s = t * c;
         for (int k = 0; k < R; ++k) {
           const double akp = A[p + k * R], akq = A[q + k * R];
           A[p + k * R] = c * akp - s * akq;
@@ -135,17 +136,25 @@ void pinv_solve_rows(const double * Gin, int R, double * X, uint64_t I) {
       }
   }
   double dmax = 0;
-  for (int i = 0; i < R; ++i) dmax = std::max(dmax, std::fabs(A[i + i * R]));
+  for (int i = 0; i < R; ++i) dmax = fmax(dmax, fabs(A[i + i * R]));
   const double cut = dmax * 2.220446049250313e-16;
-  std::vector<double> P((size_t)R * R, 0.0);
+  for (int x = 0; x < R * R; ++x) P[x] = 0.0;
   int erank = 0;
   for (int e = 0; e < R; ++e) {
     const double d = A[e + e * R];
-    if (std::fabs(d) <= cut) continue;
+    if (fabs(d) <= cut) continue;
     ++erank;
     for (int i = 0; i < R; ++i)
       for (int j = 0; j < R; ++j) P[j + i * R] += V[e + i * R] * V[e + j * R] / d;
   }
+  return erank;
+}
+
+// Minimum-norm least squares for a symmetric (possibly singular) G: the role of
+// the reference's GELSS fallback (src/matrix.c:566-603).
+void pinv_solve_rows(const double * Gin, int R, double * X, uint64_t I) {
+  std::vector<double> A(Gin, Gin + (size_t)R * R), V((size_t)R * R), P((size_t)R * R);
+  const int erank = jacobi_pinv(A.data(), V.data(), R, P.data());
   printf("SPLATT:   pseudo-inverse effective rank: %d\n", erank);
 #pragma omp parallel
   {
@@ -187,12 +196,11 @@ void normalize_cols(double * A, uint64_t I, int R, double * lambda, bool two_nor
 }
 
 // reference: p_kruskal_norm src/cpd.c:116-152
-double kruskal_norm(const std::vector<std::vector<double>> & ata, const double * lambda, int N,
-                    int R) {
+double kruskal_norm(const double * ata, const double * lambda, int N, int R) {
   std::vector<double> av((size_t)R * R, 1.0);
   for (int m = 0; m < N; ++m)
     for (int i = 0; i < R; ++i)
-      for (int j = i; j < R; ++j) av[j + i * R] *= ata[m][j + i * R];
+      for (int j = i; j < R; ++j) av[j + i * R] *= ata[(size_t)m * R * R + j + i * R];
   double nm = 0;
   for (int i = 0; i < R; ++i) {
     nm += av[i + i * R] * lambda[i] * lambda[i];
@@ -219,7 +227,18 @@ double kruskal_inner(const double * last, const double * m1, uint64_t I, int R,
   return inner;
 }
 
-double csf_frobsq(const splatt_csf * t) {   // reference: src/csf.c:817-851
+// fit = 1 - ||X - K|| / ||X||  (reference: p_calc_fit src/cpd.c:237-265)
+double cpd_fit(const double * ata, const double * lambda, int N, int R, double ttnormsq,
+               double inner) {
+  const double norm_mats = kruskal_norm(ata, lambda, N, R);
+  double residual = ttnormsq + norm_mats - 2 * inner;
+  if (residual > 0.) residual = std::sqrt(residual);
+  return 1 - residual / std::sqrt(ttnormsq);
+}
+
+}  // namespace
+
+double spb200_csf_frobsq(const splatt_csf * t) {   // reference: src/csf.c:817-851
   double norm = 0;
   const int N = (int)t->nmodes;
   for (uint64_t tile = 0; tile < t->ntiles; ++tile) {
@@ -232,18 +251,55 @@ double csf_frobsq(const splatt_csf * t) {   // reference: src/csf.c:817-851
   return norm;
 }
 
+AlsIterations::AlsIterations(const double * options)
+    : niters((uint64_t)options[SPLATT_OPTION_NITER]), tol(options[SPLATT_OPTION_TOLERANCE]),
+      verbosity((int)options[SPLATT_OPTION_VERBOSITY]) {}
 
-}  // namespace
+void AlsIterations::start() { t0 = std::chrono::steady_clock::now(); }
 
-// shared with the multi-GPU driver (multi.cu)
-double spb200_cpd_rand_val() { return rand_val(); }
-double spb200_csf_frobsq(const splatt_csf * t) { return csf_frobsq(t); }
-// post-process (src/cpd.c:391-411): 2-normalise every factor into lambda
-void spb200_cpd_postprocess(double ** mats, const uint64_t * dims, int N, int R, double * lambda) {
+bool AlsIterations::done(uint64_t it, double fit) {
+  if (verbosity > SPLATT_VERBOSITY_NONE)
+    printf("  its = %3llu (%0.3fs)  fit = %0.5f  delta = %+0.4e\n", (unsigned long long)it + 1,
+           std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count(), fit,
+           fit - oldfit);
+  if (fit == 1. || (it > 0 && std::fabs(fit - oldfit) < tol)) return true;
+  oldfit = fit;
+  return false;
+}
+
+HostKruskal::~HostKruskal() {
+  for (int m = 0; m < N; ++m) free(mats[m]);
+  free(lambda);
+}
+
+bool HostKruskal::start(int N_, const uint64_t * dims_, int R_) {
+  N = N_; R = R_;
+  memcpy(dims, dims_, sizeof(uint64_t) * N);
+  lambda = static_cast<double *>(malloc(sizeof(double) * R));
+  bool ok = lambda != nullptr;
+  for (int m = 0; m < N && ok; ++m) {
+    mats[m] = static_cast<double *>(malloc(sizeof(double) * dims[m] * R));
+    ok = mats[m] != nullptr;
+    if (ok) for (uint64_t x = 0; x < dims[m] * (uint64_t)R; ++x) mats[m][x] = rand_val();
+  }
+  return ok;
+}
+
+void HostKruskal::finish(double fit, splatt_kruskal * out) {
   std::vector<double> tmp(R);
   for (int m = 0; m < N; ++m) {
     normalize_cols(mats[m], dims[m], R, tmp.data(), true);
     for (int f = 0; f < R; ++f) lambda[f] *= tmp[f];
+  }
+  out->fit = fit;
+  out->rank = (splatt_idx_t)R;
+  out->nmodes = (splatt_idx_t)N;
+  out->lambda = lambda;
+  lambda = nullptr;
+  for (int m = 0; m < N; ++m) {
+    out->dims[m] = dims[m];
+    out->factors[m] = mats[m];
+    mats[m] = nullptr;
   }
 }
 
@@ -331,47 +387,10 @@ __global__ void k_form_chol(const double * __restrict__ ata, int nmodes, int mod
     if (threadIdx.x == 0) *info = 0;
     return;
   }
-  // not SPD: Jacobi eigen-decomposition -> pseudo-inverse (one thread; rare path)
+  // not SPD: pseudo-inverse of the unfactored matrix (one thread; rare path)
   if (threadIdx.x == 0) {
-    double * A2 = a;            // reuse as the working symmetric matrix
-    double * V  = Vscratch;
-    for (int x = 0; x < R * R; ++x) { A2[x] = Pout[x]; V[x] = 0.0; }
-    for (int i = 0; i < R; ++i) V[i + i * R] = 1.0;
-    for (int sweep = 0; sweep < 64; ++sweep) {
-      double off = 0;
-      for (int p = 0; p < R; ++p) for (int q = p + 1; q < R; ++q) off += A2[q + p * R] * A2[q + p * R];
-      if (off < 1e-300) break;
-      for (int p = 0; p < R; ++p)
-        for (int q = p + 1; q < R; ++q) {
-          const double apq = A2[q + p * R];
-          if (fabs(apq) < 1e-300) continue;
-          const double theta = (A2[q + q * R] - A2[p + p * R]) / (2.0 * apq);
-          const double t = (theta >= 0 ? 1.0 : -1.0) / (fabs(theta) + sqrt(theta * theta + 1.0));
-          const double c = 1.0 / sqrt(t * t + 1.0), sn = t * c;
-          for (int k = 0; k < R; ++k) {
-            const double akp = A2[p + k * R], akq = A2[q + k * R];
-            A2[p + k * R] = c * akp - sn * akq; A2[q + k * R] = sn * akp + c * akq;
-          }
-          for (int k = 0; k < R; ++k) {
-            const double apk = A2[k + p * R], aqk = A2[k + q * R];
-            A2[k + p * R] = c * apk - sn * aqk; A2[k + q * R] = sn * apk + c * aqk;
-          }
-          for (int k = 0; k < R; ++k) {
-            const double vkp = V[p + k * R], vkq = V[q + k * R];
-            V[p + k * R] = c * vkp - sn * vkq; V[q + k * R] = sn * vkp + c * vkq;
-          }
-        }
-    }
-    double dmax = 0;
-    for (int i = 0; i < R; ++i) dmax = fmax(dmax, fabs(A2[i + i * R]));
-    const double cut = dmax * 2.220446049250313e-16;
-    for (int x = 0; x < R * R; ++x) Pout[x] = 0.0;
-    for (int e = 0; e < R; ++e) {
-      const double d = A2[e + e * R];
-      if (fabs(d) <= cut) continue;
-      for (int i = 0; i < R; ++i)
-        for (int j = 0; j < R; ++j) Pout[j + i * R] += V[e + i * R] * V[e + j * R] / d;
-    }
+    for (int x = 0; x < R * R; ++x) a[x] = Pout[x];
+    jacobi_pinv(a, Vscratch, R, Pout);
     *info = 1;
   }
 }
@@ -533,8 +552,10 @@ k_solve_rows_reg(const T * __restrict__ M1, T * __restrict__ X, unsigned long lo
 // 64-row tiles of A through shared memory; two teams of threads (even / odd tile rows) each
 // hold the 4x4 blocks of the upper triangle of G in registers (one block per thread) and
 // flush them with one round of atomics per CTA.  reference: mat_aTa src/matrix.c:414-455
+template <int RT>
+constexpr int kSyrkThreads = 2 * ((RT / 4) * (RT / 4 + 1) / 2 + 31) / 32 * 32;   // two teams
 template <int RT, class T>
-__global__ void __launch_bounds__(2 * ((RT / 4) * (RT / 4 + 1) / 2 + 31) / 32 * 32)
+__global__ void __launch_bounds__(kSyrkThreads<RT>)
 k_gram_syrk(const T * __restrict__ A, unsigned long long I, int R, int lda,
             double * __restrict__ G) {
   constexpr int NB     = RT / 4;                       // 4x4 blocks per side
@@ -631,6 +652,18 @@ __global__ void k_scale_cols(T * __restrict__ A, unsigned long long I, int R, in
   const int j = (int)(x % R);
   A[i * ld + j] = static_cast<T>(static_cast<double>(A[i * ld + j]) / lambda[j]);
 }
+// *out += the sum of v over the block (whole warps): warp shuffles, then one atomic per block
+__device__ __forceinline__ void block_sum_add(double v, double * out) {
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  __shared__ double red[32];
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+  __syncthreads();
+  if (threadIdx.x < 32) {
+    v = threadIdx.x < blockDim.x / 32 ? red[threadIdx.x] : 0.0;
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    if (threadIdx.x == 0) atomicAdd(out, v);
+  }
+}
 // inner += sum_i sum_r A[i,r] * M1[i,r] * lambda[r].  reference: p_tt_kruskal_inner src/cpd.c:171-218
 template <class T>
 __global__ void k_inner(const T * __restrict__ A, const T * __restrict__ M1,
@@ -643,15 +676,7 @@ __global__ void k_inner(const T * __restrict__ A, const T * __restrict__ M1,
     const int j = (int)(x % R);
     v = fma(static_cast<double>(A[i * ld + j]) * static_cast<double>(M1[i * ld + j]), lambda[j], v);
   }
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  __shared__ double red[32];
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
-  __syncthreads();
-  if (threadIdx.x < 32) {
-    v = threadIdx.x < blockDim.x / 32 ? red[threadIdx.x] : 0.0;
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    if (threadIdx.x == 0) atomicAdd(inner, v);
-  }
+  block_sum_add(v, inner);
 }
 
 // ||X||^2 as an fp64 sum of squares over one stream's record values: the device CPD entries
@@ -664,15 +689,7 @@ __global__ void k_vals_sumsq(const SpRec * __restrict__ rec, unsigned long long 
     const double a = rec[x].v;
     v = fma(a, a, v);
   }
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  __shared__ double red[32];
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
-  __syncthreads();
-  if (threadIdx.x < 32) {
-    v = threadIdx.x < blockDim.x / 32 ? red[threadIdx.x] : 0.0;
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    if (threadIdx.x == 0) atomicAdd(out, v);
-  }
+  block_sum_add(v, out);
 }
 // post-processing (src/cpd.c:391-411): lambda_total *= the column 2-norms just divided out
 __global__ void k_fold_lambda(double * __restrict__ lambda_total, const double * __restrict__ norms,
@@ -723,6 +740,14 @@ __global__ void k_sum_partials(const double * __restrict__ parts, int k, int str
   dst[x] = v;
 }
 
+// f(std::integral_constant<int, RT>()) for the register tile rt = 16, 32 or 64
+template <class F>
+void with_rt(int rt, F && f) {
+  if (rt == 16) f(std::integral_constant<int, 16>());
+  else if (rt == 32) f(std::integral_constant<int, 32>());
+  else f(std::integral_constant<int, 64>());
+}
+
 struct DevTail {
   int N = 0, R = 0, ld = 0;
   double * ata = nullptr;     // N x R x R
@@ -749,12 +774,11 @@ struct DevTail {
     if (ok && rt) {
       const int sb = (2 * rt * rt + rt) * 8, gb = 64 * rt * 8;
       cudaError_t e1 = cudaSuccess, e2 = cudaSuccess;
-      if (rt == 16) { e1 = cudaFuncSetAttribute(k_solve_rows_reg<16, T>, cudaFuncAttributeMaxDynamicSharedMemorySize, sb);
-                      e2 = cudaFuncSetAttribute(k_gram_syrk<16, T>, cudaFuncAttributeMaxDynamicSharedMemorySize, gb); }
-      if (rt == 32) { e1 = cudaFuncSetAttribute(k_solve_rows_reg<32, T>, cudaFuncAttributeMaxDynamicSharedMemorySize, sb);
-                      e2 = cudaFuncSetAttribute(k_gram_syrk<32, T>, cudaFuncAttributeMaxDynamicSharedMemorySize, gb); }
-      if (rt == 64) { e1 = cudaFuncSetAttribute(k_solve_rows_reg<64, T>, cudaFuncAttributeMaxDynamicSharedMemorySize, sb);
-                      e2 = cudaFuncSetAttribute(k_gram_syrk<64, T>, cudaFuncAttributeMaxDynamicSharedMemorySize, gb); }
+      with_rt(rt, [&](auto c) {
+        constexpr int RT = decltype(c)::value;
+        e1 = cudaFuncSetAttribute(k_solve_rows_reg<RT, T>, cudaFuncAttributeMaxDynamicSharedMemorySize, sb);
+        e2 = cudaFuncSetAttribute(k_gram_syrk<RT, T>, cudaFuncAttributeMaxDynamicSharedMemorySize, gb);
+      });
       if (e1 != cudaSuccess || e2 != cudaSuccess) { cudaGetLastError(); rt = 0; }
     }
     return ok;
@@ -817,9 +841,10 @@ struct DevTail {
     if (rt && I >= 32768) {
       const unsigned blocks = (unsigned)std::min<uint64_t>((I + 63) / 64, 296);
       const size_t sm = (size_t)64 * rt * 8;
-      if (rt == 16) k_gram_syrk<16, T><<<blocks, 64, sm, s>>>(A, I, R, ld, G);
-      else if (rt == 32) k_gram_syrk<32, T><<<blocks, 128, sm, s>>>(A, I, R, ld, G);
-      else k_gram_syrk<64, T><<<blocks, 320, sm, s>>>(A, I, R, ld, G);
+      with_rt(rt, [&](auto c) {
+        constexpr int RT = decltype(c)::value;
+        k_gram_syrk<RT, T><<<blocks, kSyrkThreads<RT>, sm, s>>>(A, I, R, ld, G);
+      });
     } else {
       const unsigned blocks = (unsigned)std::min<uint64_t>((I + 31) / 32, 592);
       k_gram<T><<<blocks, 256, 32 * R * 8, s>>>(A, I, R, ld, G);
@@ -852,9 +877,9 @@ struct DevTail {
       // register-tiled solve when the Cholesky succeeded (it returns at once otherwise) ...
       const size_t sm = (size_t)(2 * rt * rt + rt) * 8;
       const unsigned nb = (unsigned)((I + 127) / 128);
-      if (rt == 16) k_solve_rows_reg<16, T><<<nb, 128, sm, s>>>(d_out, d_mat, I, R, ld, chol, info);
-      else if (rt == 32) k_solve_rows_reg<32, T><<<nb, 128, sm, s>>>(d_out, d_mat, I, R, ld, chol, info);
-      else k_solve_rows_reg<64, T><<<nb, 128, sm, s>>>(d_out, d_mat, I, R, ld, chol, info);
+      with_rt(rt, [&](auto c) {
+        k_solve_rows_reg<decltype(c)::value, T><<<nb, 128, sm, s>>>(d_out, d_mat, I, R, ld, chol, info);
+      });
       // ... and the generic kernel only for the pseudo-inverse fallback (info != 0)
       k_solve_rows<T><<<(unsigned)((I + NT - 1) / NT), NT, (R * R + R * NT) * 8, s>>>(
           d_out, d_mat, I, R, ld, chol, pinv, info, 1);
@@ -884,6 +909,29 @@ struct DevTail {
       check("post-process");
       spb200_count_launches(I ? 4 : 2);
     }
+  }
+
+  // Fit after the last mode's update from its factor and M1 (reference: p_calc_fit
+  // src/cpd.c:237-265): inner product on the device, one read-back of the Grams, lambda and
+  // the inner product (and the solver info when info_out is set), synchronising the stream.
+  // lambda_out (R host doubles) and info_out may be null.  Check `failed` afterwards: when it
+  // is set (by this synchronisation or an earlier launch) nothing has been written.
+  template <class T>
+  double fit(const T * last, const T * m1, uint64_t rows, double ttnormsq, double * lambda_out,
+             int * info_out) {
+    const size_t nb = (size_t)N * R * R;
+    cudaMemsetAsync(inner, 0, sizeof(double), s);
+    k_inner<T><<<296, 256, 0, s>>>(last, m1, rows, R, ld, lambda, inner);
+    spb200_count_launches(1);
+    cudaMemcpyAsync(h_back, ata, nb * 8, cudaMemcpyDeviceToHost, s);
+    cudaMemcpyAsync(h_back + nb, lambda, R * 8, cudaMemcpyDeviceToHost, s);
+    cudaMemcpyAsync(h_back + nb + R, inner, 8, cudaMemcpyDeviceToHost, s);
+    if (info_out) cudaMemcpyAsync(h_back + nb + R + 1, info, 4, cudaMemcpyDeviceToHost, s);
+    if (cudaStreamSynchronize(s) != cudaSuccess) failed = true;
+    if (failed) return 0.0;
+    if (lambda_out) memcpy(lambda_out, h_back + nb, sizeof(double) * R);
+    if (info_out) memcpy(info_out, h_back + nb + R + 1, sizeof(int));
+    return cpd_fit(h_back, h_back + nb, N, R, ttnormsq, h_back[nb + R]);
   }
 
   // ---- row-partitioned tail (see the kernels above)
@@ -922,15 +970,6 @@ struct DevTail {
   }
 };
 
-// fit = 1 - ||X - K|| / ||X||  (reference: p_calc_fit src/cpd.c:237-265)
-double cpd_fit(const std::vector<std::vector<double>> & ata, const double * lambda, int N, int R,
-               double ttnormsq, double inner) {
-  const double norm_mats = kruskal_norm(ata, lambda, N, R);
-  double residual = ttnormsq + norm_mats - 2 * inner;
-  if (residual > 0.) residual = std::sqrt(residual);
-  return 1 - residual / std::sqrt(ttnormsq);
-}
-
 int mttkrp_t(const splatt_b200_tensor * t, int m, int R, int ldm, double * const * d_mats,
              double * d_out, cudaStream_t s) {
   return splatt_b200_mttkrp(t, m, R, ldm, d_mats, d_out, s);
@@ -952,47 +991,25 @@ bool run_device_als(const splatt_b200_tensor * t, T * const * d_mats, T * d_out,
                     double * fit_out, uint64_t * iterations_out) {
   const int N = tail.N, R = tail.R;
   const uint64_t * dims = t->dims;
-  const cudaStream_t stream = tail.s;
-  const int verbosity = (int)options[SPLATT_OPTION_VERBOSITY];
-  const uint64_t niters = (uint64_t)options[SPLATT_OPTION_NITER];
-  std::vector<std::vector<double>> ata(N, std::vector<double>((size_t)R * R));
-  double fit = 0, oldfit = 0;
+  AlsIterations iters(options);
+  double fit = 0;
   uint64_t its = 0;
   bool ok = true;
   for (int m = 0; m < N; ++m) tail.gram(d_mats[m], dims[m], m);
-  const size_t nb = (size_t)N * R * R;
-  for (uint64_t it = 0; it < niters && ok; ++it) {
-    auto t0 = std::chrono::steady_clock::now();
+  for (uint64_t it = 0; it < iters.niters && ok; ++it) {
+    iters.start();
     for (int m = 0; m < N && ok; ++m) {
-      if (mttkrp_t(t, m, R, ldm, d_mats, d_out, stream) != SPLATT_SUCCESS) { ok = false; break; }
+      if (mttkrp_t(t, m, R, ldm, d_mats, d_out, tail.s) != SPLATT_SUCCESS) { ok = false; break; }
       tail.mode_step(d_out, d_mats[m], dims[m], m, it == 0);
     }
     if (!ok) break;
-    cudaMemsetAsync(tail.inner, 0, sizeof(double), stream);
-    k_inner<T><<<296, 256, 0, stream>>>(d_mats[N - 1], d_out, dims[N - 1], R, ldm, tail.lambda,
-                                        tail.inner);
-    spb200_count_launches(1);
-    cudaMemcpyAsync(tail.h_back, tail.ata, nb * 8, cudaMemcpyDeviceToHost, stream);
-    cudaMemcpyAsync(tail.h_back + nb, tail.lambda, R * 8, cudaMemcpyDeviceToHost, stream);
-    cudaMemcpyAsync(tail.h_back + nb + R, tail.inner, 8, cudaMemcpyDeviceToHost, stream);
-    cudaMemcpyAsync(tail.h_back + nb + R + 1, tail.info, 4, cudaMemcpyDeviceToHost, stream);
-    if (cudaStreamSynchronize(stream) != cudaSuccess || tail.failed) { ok = false; break; }
-    for (int m = 0; m < N; ++m)
-      memcpy(ata[m].data(), tail.h_back + (size_t)m * R * R, sizeof(double) * R * R);
-    memcpy(lambda, tail.h_back + nb, sizeof(double) * R);
     int info_last = 0;
-    memcpy(&info_last, tail.h_back + nb + R + 1, sizeof(int));
+    fit = tail.fit(d_mats[N - 1], d_out, dims[N - 1], ttnormsq, lambda, &info_last);
+    if (tail.failed) { ok = false; break; }
     if (info_last)
       fprintf(stderr, "SPLATT: Gram matrix is not SPD. Used pseudo-inverse.\n");
-    fit = cpd_fit(ata, lambda, N, R, ttnormsq, tail.h_back[nb + R]);
     its = it + 1;
-    if (verbosity > SPLATT_VERBOSITY_NONE)
-      printf("  its = %3llu (%0.3fs)  fit = %0.5f  delta = %+0.4e\n", (unsigned long long)it + 1,
-             std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count(), fit,
-             fit - oldfit);
-    if (fit == 1. || (it > 0 && std::fabs(fit - oldfit) < options[SPLATT_OPTION_TOLERANCE]))
-      break;
-    oldfit = fit;
+    if (iters.done(it, fit)) break;
   }
   *fit_out = fit;
   *iterations_out = its;
@@ -1115,35 +1132,20 @@ int splatt_cpd_als(splatt_csf const * const tensors, splatt_idx_t const nfactors
   if (rc != SPLATT_SUCCESS) return rc;
 
   // factor matrices: random init in the reference's draw order (src/cpd.c:36-40)
-  double * mats[SPB200_MAXN] = {nullptr};
+  HostKruskal K;
   double * d_mats[SPB200_MAXN] = {nullptr};
   double * d_out = nullptr;
   double * m1 = nullptr;          // pinned MTTKRP result (host tail only)
-  double * lambda = static_cast<double *>(malloc(sizeof(double) * R));
   cudaStream_t stream = nullptr;
   DevTail tail;
-  bool ok = lambda != nullptr;
-  for (int m = 0; m < N && ok; ++m) {
-    mats[m] = static_cast<double *>(malloc(sizeof(double) * dims[m] * R));
-    ok = mats[m] != nullptr;
-    if (ok) for (uint64_t x = 0; x < dims[m] * (uint64_t)R; ++x) mats[m][x] = rand_val();
-  }
-  auto h2d = [&](int m) -> cudaError_t {
-    if (ldm == R) return cudaMemcpyAsync(d_mats[m], mats[m], dims[m] * (size_t)R * 8,
-                                         cudaMemcpyHostToDevice, stream);
-    return cudaMemcpy2DAsync(d_mats[m], (size_t)ldm * 8, mats[m], (size_t)R * 8, (size_t)R * 8,
-                             dims[m], cudaMemcpyHostToDevice, stream);
-  };
-  auto d2h = [&](double * dst, const double * src, uint64_t I) -> cudaError_t {
-    if (ldm == R) return cudaMemcpyAsync(dst, src, I * (size_t)R * 8, cudaMemcpyDeviceToHost, stream);
-    return cudaMemcpy2DAsync(dst, (size_t)R * 8, src, (size_t)ldm * 8, (size_t)R * 8, I,
-                             cudaMemcpyDeviceToHost, stream);
-  };
+  bool ok = K.start(N, dims, R);
+  double ** mats = K.mats;
+  double * lambda = K.lambda;
   ok = ok && cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking) == cudaSuccess;
   for (int m = 0; m < N && ok; ++m) {
     ok = cudaMalloc(&d_mats[m], dims[m] * (size_t)ldm * 8) == cudaSuccess &&
          cudaMemsetAsync(d_mats[m], 0, dims[m] * (size_t)ldm * 8, stream) == cudaSuccess &&
-         h2d(m) == cudaSuccess;
+         h2d_matrix(d_mats[m], ldm, mats[m], dims[m], R, stream) == cudaSuccess;
   }
   ok = ok && cudaMalloc(&d_out, maxdim * (size_t)ldm * 8) == cudaSuccess;
   if (host_tail) ok = ok && cudaMallocHost(&m1, maxdim * (size_t)R * 8) == cudaSuccess;
@@ -1151,31 +1153,25 @@ int splatt_cpd_als(splatt_csf const * const tensors, splatt_idx_t const nfactors
   if (ok && !host_tail && verbosity > SPLATT_VERBOSITY_LOW)
     printf("SPLATT-B200: device ALS tail, %d rows per solve block\n", tail.solve_threads);
 
-  double fit = 0, oldfit = 0;
-  const double ttnormsq = csf_frobsq(tensors);
-  const uint64_t niters = (uint64_t)options[SPLATT_OPTION_NITER];
-  std::vector<std::vector<double>> ata(N, std::vector<double>((size_t)R * R));
-  auto report = [&](uint64_t it, double secs) {
-    if (verbosity > SPLATT_VERBOSITY_NONE)
-      printf("  its = %3llu (%0.3fs)  fit = %0.5f  delta = %+0.4e\n", (unsigned long long)it + 1,
-             secs, fit, fit - oldfit);
-  };
-  auto fit_from = [&](double inner) { fit = cpd_fit(ata, lambda, N, R, ttnormsq, inner); };
+  double fit = 0;
+  const double ttnormsq = spb200_csf_frobsq(tensors);
 
   if (ok && host_tail) {
-    for (int m = 0; m < N; ++m) gram(mats[m], dims[m], R, ata[m].data());
+    AlsIterations iters(options);
+    std::vector<double> ata((size_t)N * R * R);
+    for (int m = 0; m < N; ++m) gram(mats[m], dims[m], R, ata.data() + (size_t)m * R * R);
     std::vector<double> neq((size_t)R * R);
-    for (uint64_t it = 0; it < niters && ok; ++it) {
-      auto t0 = std::chrono::steady_clock::now();
+    for (uint64_t it = 0; it < iters.niters && ok; ++it) {
+      iters.start();
       for (int m = 0; m < N && ok; ++m) {
         // M1 = X_(m) (khatri-rao of the other factors), on the GPU
         rc = splatt_b200_mttkrp(T, m, R, ldm, d_mats, d_out, stream);
-        cudaError_t e = d2h(m1, d_out, dims[m]);
+        cudaError_t e = d2h_matrix(m1, d_out, ldm, dims[m], R, stream);
         if (e == cudaSuccess) e = cudaStreamSynchronize(stream);
         if (rc != SPLATT_SUCCESS || e != cudaSuccess) { ok = false; break; }
         // A_m = M1 * (hadamard Grams)^-1   (src/cpd.c:337-339, src/matrix.c:529-606)
         memcpy(mats[m], m1, dims[m] * (size_t)R * 8);
-        form_normal_matrix(ata, m, N, R, neq.data());
+        form_normal_matrix(ata.data(), m, N, R, neq.data());
         std::vector<double> chol(neq);
         if (cholesky(chol.data(), R)) {
           cholesky_solve_rows(chol.data(), R, mats[m], dims[m]);
@@ -1184,25 +1180,23 @@ int splatt_cpd_als(splatt_csf const * const tensors, splatt_idx_t const nfactors
           pinv_solve_rows(neq.data(), R, mats[m], dims[m]);
         }
         normalize_cols(mats[m], dims[m], R, lambda, it == 0);   // src/cpd.c:343-347
-        gram(mats[m], dims[m], R, ata[m].data());               // src/cpd.c:350
-        ok = h2d(m) == cudaSuccess;                             // keep the device copy current
+        gram(mats[m], dims[m], R, ata.data() + (size_t)m * R * R);   // src/cpd.c:350
+        // keep the device copy current
+        ok = h2d_matrix(d_mats[m], ldm, mats[m], dims[m], R, stream) == cudaSuccess;
       }
       if (!ok) break;
-      fit_from(kruskal_inner(mats[N - 1], m1, dims[N - 1], R, lambda));
-      report(it, std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count());
-      if (fit == 1. || (it > 0 && std::fabs(fit - oldfit) < options[SPLATT_OPTION_TOLERANCE]))
-        break;
-      oldfit = fit;
+      const double inner = kruskal_inner(mats[N - 1], m1, dims[N - 1], R, lambda);
+      fit = cpd_fit(ata.data(), lambda, N, R, ttnormsq, inner);
+      if (iters.done(it, fit)) break;
     }
   } else if (ok) {
     // ---- everything on the device; one small read-back per iteration for the fit
     uint64_t its = 0;
     ok = run_device_als<double>(T, d_mats, d_out, ldm, tail, ttnormsq, options, lambda, &fit, &its);
-    for (int m = 0; m < N && ok; ++m) ok = d2h(mats[m], d_mats[m], dims[m]) == cudaSuccess;
+    for (int m = 0; m < N && ok; ++m)
+      ok = d2h_matrix(mats[m], d_mats[m], ldm, dims[m], R, stream) == cudaSuccess;
     ok = ok && cudaStreamSynchronize(stream) == cudaSuccess;
   }
-  // post-process (src/cpd.c:391-411): 2-normalise every factor into lambda
-  if (ok) spb200_cpd_postprocess(mats, dims, N, R, lambda);
   if (stream) cudaStreamSynchronize(stream);
   for (int m = 0; m < N; ++m) if (d_mats[m]) cudaFree(d_mats[m]);
   if (d_out) cudaFree(d_out);
@@ -1212,18 +1206,9 @@ int splatt_cpd_als(splatt_csf const * const tensors, splatt_idx_t const nfactors
   splatt_b200_tensor_free(T);
   if (!ok) {
     fprintf(stderr, "SPLATT: CPD-ALS failed (%s)\n", cudaGetErrorString(cudaGetLastError()));
-    for (int m = 0; m < N; ++m) free(mats[m]);
-    free(lambda);
     return SPLATT_ERROR_NOMEMORY;
   }
-  factored->fit = fit;
-  factored->rank = nfactors;
-  factored->nmodes = N;
-  factored->lambda = lambda;
-  for (int m = 0; m < N; ++m) {
-    factored->dims[m] = dims[m];
-    factored->factors[m] = mats[m];
-  }
+  K.finish(fit, factored);     // post-process (src/cpd.c:391-411)
   return SPLATT_SUCCESS;
 }
 
@@ -1239,25 +1224,27 @@ struct splatt_b200_als_tail { DevTail t; };
 namespace {
 
 template <class T>
+int tail_gram(splatt_b200_als_tail * h, int mode, const T * d_factor, uint64_t rows) {
+  if (!h || mode < 0 || mode >= h->t.N) return SPLATT_ERROR_BADINPUT;
+  h->t.gram(d_factor, rows, mode);
+  return (cudaGetLastError() == cudaSuccess && !h->t.failed) ? SPLATT_SUCCESS : SPLATT_ERROR_BADINPUT;
+}
+
+template <class T>
+int tail_update(splatt_b200_als_tail * h, int mode, const T * d_m1, T * d_factor, uint64_t rows,
+                int first_iteration) {
+  if (!h || mode < 0 || mode >= h->t.N) return SPLATT_ERROR_BADINPUT;
+  h->t.mode_step(d_m1, d_factor, rows, mode, first_iteration != 0);
+  return (cudaGetLastError() == cudaSuccess && !h->t.failed) ? SPLATT_SUCCESS : SPLATT_ERROR_BADINPUT;
+}
+
+template <class T>
 int tail_fit(splatt_b200_als_tail * h, const T * d_last_factor, const T * d_last_m1, uint64_t rows,
              double ttnormsq, double * fit_out, double * lambda_out) {
   if (!h || !fit_out) return SPLATT_ERROR_BADINPUT;
-  DevTail & t = h->t;
-  const int N = t.N, R = t.R;
-  const size_t nb = (size_t)N * R * R;
-  cudaMemsetAsync(t.inner, 0, sizeof(double), t.s);
-  k_inner<T><<<296, 256, 0, t.s>>>(d_last_factor, d_last_m1, rows, R, t.ld, t.lambda, t.inner);
-  spb200_count_launches(1);
-  cudaMemcpyAsync(t.h_back, t.ata, nb * 8, cudaMemcpyDeviceToHost, t.s);
-  cudaMemcpyAsync(t.h_back + nb, t.lambda, R * 8, cudaMemcpyDeviceToHost, t.s);
-  cudaMemcpyAsync(t.h_back + nb + R, t.inner, 8, cudaMemcpyDeviceToHost, t.s);
-  if (cudaStreamSynchronize(t.s) != cudaSuccess || t.failed) return SPLATT_ERROR_BADINPUT;
-  std::vector<std::vector<double>> ata(N, std::vector<double>((size_t)R * R));
-  for (int m = 0; m < N; ++m)
-    memcpy(ata[m].data(), t.h_back + (size_t)m * R * R, sizeof(double) * R * R);
-  const double * lambda = t.h_back + nb;
-  *fit_out = cpd_fit(ata, lambda, N, R, ttnormsq, t.h_back[nb + R]);
-  if (lambda_out) memcpy(lambda_out, lambda, sizeof(double) * R);
+  const double fit = h->t.fit(d_last_factor, d_last_m1, rows, ttnormsq, lambda_out, nullptr);
+  if (h->t.failed) return SPLATT_ERROR_BADINPUT;
+  *fit_out = fit;
   return SPLATT_SUCCESS;
 }
 
@@ -1294,17 +1281,13 @@ void splatt_b200_als_tail_free(splatt_b200_als_tail * h) {
 // Gram of one factor (call once per factor before the first iteration).
 int splatt_b200_als_tail_gram(splatt_b200_als_tail * h, int mode, double const * d_factor,
                               uint64_t rows) {
-  if (!h || mode < 0 || mode >= h->t.N) return SPLATT_ERROR_BADINPUT;
-  h->t.gram(d_factor, rows, mode);
-  return (cudaGetLastError() == cudaSuccess && !h->t.failed) ? SPLATT_SUCCESS : SPLATT_ERROR_BADINPUT;
+  return tail_gram(h, mode, d_factor, rows);
 }
 
 // One mode update: d_m1 (the summed MTTKRP result) -> d_factor, lambda, Gram of the mode.
 int splatt_b200_als_tail_update(splatt_b200_als_tail * h, int mode, double const * d_m1,
                                 double * d_factor, uint64_t rows, int first_iteration) {
-  if (!h || mode < 0 || mode >= h->t.N) return SPLATT_ERROR_BADINPUT;
-  h->t.mode_step(d_m1, d_factor, rows, mode, first_iteration != 0);
-  return (cudaGetLastError() == cudaSuccess && !h->t.failed) ? SPLATT_SUCCESS : SPLATT_ERROR_BADINPUT;
+  return tail_update(h, mode, d_m1, d_factor, rows, first_iteration);
 }
 
 // Fit after the last mode's update (reference: p_calc_fit src/cpd.c:237-265).  Synchronises
@@ -1317,16 +1300,14 @@ int splatt_b200_als_tail_fit(splatt_b200_als_tail * h, double const * d_last_fac
 
 int splatt_b200_als_tail_gram_f32(splatt_b200_als_tail * h, int mode, float const * d_factor,
                                   uint64_t rows) {
-  if (!f32_tail_ok(h, d_factor, d_factor) || mode < 0 || mode >= h->t.N) return SPLATT_ERROR_BADINPUT;
-  h->t.gram(d_factor, rows, mode);
-  return (cudaGetLastError() == cudaSuccess && !h->t.failed) ? SPLATT_SUCCESS : SPLATT_ERROR_BADINPUT;
+  if (!f32_tail_ok(h, d_factor, d_factor)) return SPLATT_ERROR_BADINPUT;
+  return tail_gram(h, mode, d_factor, rows);
 }
 
 int splatt_b200_als_tail_update_f32(splatt_b200_als_tail * h, int mode, float const * d_m1,
                                     float * d_factor, uint64_t rows, int first_iteration) {
-  if (!f32_tail_ok(h, d_m1, d_factor) || mode < 0 || mode >= h->t.N) return SPLATT_ERROR_BADINPUT;
-  h->t.mode_step(d_m1, d_factor, rows, mode, first_iteration != 0);
-  return (cudaGetLastError() == cudaSuccess && !h->t.failed) ? SPLATT_SUCCESS : SPLATT_ERROR_BADINPUT;
+  if (!f32_tail_ok(h, d_m1, d_factor)) return SPLATT_ERROR_BADINPUT;
+  return tail_update(h, mode, d_m1, d_factor, rows, first_iteration);
 }
 
 int splatt_b200_als_tail_fit_f32(splatt_b200_als_tail * h, float const * d_last_factor,

@@ -102,18 +102,6 @@ void free_priv(WsPriv * w) {
   free(w);
 }
 
-// Copy a host row-major I x J matrix into a device I x ldm buffer.
-cudaError_t h2d_matrix(double * dst, int ldm, const double * src, uint64_t I, uint64_t J,
-                       cudaStream_t s) {
-  if ((uint64_t)ldm == J) return cudaMemcpyAsync(dst, src, I * J * 8, cudaMemcpyHostToDevice, s);
-  return cudaMemcpy2DAsync(dst, (size_t)ldm * 8, src, J * 8, J * 8, I, cudaMemcpyHostToDevice, s);
-}
-cudaError_t d2h_matrix(double * dst, const double * src, int ldm, uint64_t I, uint64_t J,
-                       cudaStream_t s) {
-  if ((uint64_t)ldm == J) return cudaMemcpyAsync(dst, src, I * J * 8, cudaMemcpyDeviceToHost, s);
-  return cudaMemcpy2DAsync(dst, J * 8, src, (size_t)ldm * 8, J * 8, I, cudaMemcpyDeviceToHost, s);
-}
-
 bool is_pinned(const void * p, size_t bytes) {
   // both ends of the range must be page-locked host memory
   cudaPointerAttributes a0, a1;

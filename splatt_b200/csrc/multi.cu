@@ -25,11 +25,6 @@
 #include <cstring>
 #include <vector>
 
-// cpd.cu
-double spb200_cpd_rand_val();
-void   spb200_cpd_postprocess(double ** mats, const uint64_t * dims, int N, int R, double * lambda);
-double spb200_csf_frobsq(const splatt_csf * t);
-
 namespace {
 
 constexpr int kMaxDev = 16;
@@ -854,37 +849,23 @@ int splatt_b200_multi_cpd_als(splatt_b200_multi * h, splatt_csf const * tensors,
     fprintf(stderr, "SPLATT: multi-GPU CPD-ALS supports rank <= 128\n");
     return SPLATT_ERROR_BADINPUT;
   }
-  const int verbosity = (int)options[SPLATT_OPTION_VERBOSITY];
   // multicast available: the tail is ROW-PARTITIONED over the devices (each solves, normalises
   // and Grams its own row slice and multicasts it); otherwise one tail on device 0 + pulls
   const char * pe = getenv("SPLATT_B200_PARTITIONED_TAIL");
   const bool part = h->multicast && !(pe && atoi(pe) == 0);
-  double * mats[SPB200_MAXN] = {nullptr};
-  double * lambda = static_cast<double *>(malloc(sizeof(double) * R));
-  bool ok = lambda != nullptr;
-  for (int m = 0; m < N && ok; ++m) {
-    mats[m] = static_cast<double *>(malloc(sizeof(double) * h->dims[m] * R));
-    ok = mats[m] != nullptr;
-    if (ok) for (uint64_t x = 0; x < h->dims[m] * (uint64_t)R; ++x) mats[m][x] = spb200_cpd_rand_val();
-  }
+  HostKruskal K;
   auto fail = [&](int rc) {
-    for (int m = 0; m < N; ++m) free(mats[m]);
-    free(lambda);
     cudaSetDevice(h->prev_dev);
     return rc;
   };
-  if (!ok) return fail(SPLATT_ERROR_NOMEMORY);
+  if (!K.start(N, h->dims, R)) return fail(SPLATT_ERROR_NOMEMORY);
   int rc = SPLATT_SUCCESS;
   for (int i = 0; i < k && rc == SPLATT_SUCCESS; ++i) {
     DevState & s = h->d[i];
     if (cudaSetDevice(s.dev) != cudaSuccess) return fail(SPLATT_ERROR_BADINPUT);
-    for (int m = 0; m < N; ++m) {
-      cudaError_t e = (ldm == R)
-          ? cudaMemcpyAsync(s.mats[m], mats[m], h->dims[m] * (size_t)R * 8, cudaMemcpyHostToDevice, s.stream)
-          : cudaMemcpy2DAsync(s.mats[m], (size_t)ldm * 8, mats[m], (size_t)R * 8, (size_t)R * 8,
-                              h->dims[m], cudaMemcpyHostToDevice, s.stream);
-      if (e != cudaSuccess) return fail(SPLATT_ERROR_BADINPUT);
-    }
+    for (int m = 0; m < N; ++m)
+      if (h2d_matrix(s.mats[m], ldm, K.mats[m], h->dims[m], R, s.stream) != cudaSuccess)
+        return fail(SPLATT_ERROR_BADINPUT);
     if (i == 0 || part) {
       if (!s.tail) rc = splatt_b200_als_tail_create(N, R, ldm, s.stream, &s.tail);
       if (!part)
@@ -949,10 +930,10 @@ int splatt_b200_multi_cpd_als(splatt_b200_multi * h, splatt_csf const * tensors,
   }
 
   const double ttnormsq = spb200_csf_frobsq(tensors);
-  const uint64_t niters = (uint64_t)options[SPLATT_OPTION_NITER];
-  double fit = 0, oldfit = 0;
-  for (uint64_t it = 0; it < niters; ++it) {
-    auto t0 = std::chrono::steady_clock::now();
+  AlsIterations iters(options);
+  double fit = 0;
+  for (uint64_t it = 0; it < iters.niters; ++it) {
+    iters.start();
     for (int m = 0; m < N; ++m) {
       if (timing) { phase_done(4); }
       if (!(part && !timing)) {
@@ -1065,16 +1046,11 @@ int splatt_b200_multi_cpd_als(splatt_b200_multi * h, splatt_csf const * tensors,
     }
     if (cudaSetDevice(h->d[0].dev) != cudaSuccess) return fail(SPLATT_ERROR_BADINPUT);
     rc = splatt_b200_als_tail_fit(h->d[0].tail, h->d[0].mats[N - 1], h->d[0].out[N - 1],
-                                  h->dims[N - 1], ttnormsq, &fit, lambda);
+                                  h->dims[N - 1], ttnormsq, &fit, K.lambda);
     if (rc != SPLATT_SUCCESS) return fail(rc);
     rc = multi_release(h, 0, N - 1);
     if (rc != SPLATT_SUCCESS) return fail(rc);
-    const double secs = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
-    if (verbosity > SPLATT_VERBOSITY_NONE)
-      printf("  its = %3llu (%0.3fs)  fit = %0.5f  delta = %+0.4e\n", (unsigned long long)it + 1,
-             secs, fit, fit - oldfit);
-    if (fit == 1. || (it > 0 && std::fabs(fit - oldfit) < options[SPLATT_OPTION_TOLERANCE])) break;
-    oldfit = fit;
+    if (iters.done(it, fit)) break;
   }
   if (timing)
     printf("SPLATT-B200: multi CPD phases (ms, all iterations): mttkrp %.2f | solve+norm %.2f | "
@@ -1084,28 +1060,16 @@ int splatt_b200_multi_cpd_als(splatt_b200_multi * h, splatt_csf const * tensors,
   {
     DevState & s = h->d[0];
     if (cudaSetDevice(s.dev) != cudaSuccess) return fail(SPLATT_ERROR_BADINPUT);
-    for (int m = 0; m < N; ++m) {
-      cudaError_t e = (ldm == R)
-          ? cudaMemcpyAsync(mats[m], s.mats[m], h->dims[m] * (size_t)R * 8, cudaMemcpyDeviceToHost, s.stream)
-          : cudaMemcpy2DAsync(mats[m], (size_t)R * 8, s.mats[m], (size_t)ldm * 8, (size_t)R * 8,
-                              h->dims[m], cudaMemcpyDeviceToHost, s.stream);
-      if (e != cudaSuccess) return fail(SPLATT_ERROR_BADINPUT);
-    }
+    for (int m = 0; m < N; ++m)
+      if (d2h_matrix(K.mats[m], s.mats[m], ldm, h->dims[m], R, s.stream) != cudaSuccess)
+        return fail(SPLATT_ERROR_BADINPUT);
   }
   for (int i = 0; i < k; ++i) {
     cudaSetDevice(h->d[i].dev);
     if (cudaStreamSynchronize(h->d[i].stream) != cudaSuccess) return fail(SPLATT_ERROR_BADINPUT);
   }
   cudaSetDevice(h->prev_dev);
-  spb200_cpd_postprocess(mats, h->dims, N, R, lambda);
-  factored->fit = fit;
-  factored->rank = (splatt_idx_t)R;
-  factored->nmodes = (splatt_idx_t)N;
-  factored->lambda = lambda;
-  for (int m = 0; m < N; ++m) {
-    factored->dims[m] = h->dims[m];
-    factored->factors[m] = mats[m];
-  }
+  K.finish(fit, factored);     // post-process (src/cpd.c:391-411)
   return SPLATT_SUCCESS;
 }
 

@@ -248,19 +248,22 @@ def test_cpd_als_tracks_reference(S, host_solve, spec, monkeypatch):
         assert np.allclose(a, b, rtol=1e-5, atol=1e-8)
 
 
-def test_cpd_als_rank_deficient_falls_back(S):
+def test_cpd_als_rank_deficient_falls_back(S, monkeypatch):
     """Duplicate factor columns cannot arise from random init, so force a singular normal
     matrix with rank > number of distinct rows: both the reference (GELSS) and we
-    (pseudo-inverse) must return a finite fit and agree."""
+    (pseudo-inverse) must return a finite fit and agree, with the dense ALS tail on the
+    device and on the host (SPLATT_B200_HOST_SOLVE=0/1)."""
     dims, inds, vals = random_coo((3, 40, 30), 600, seed=9)
     dims, inds, vals = cover_all_slices(dims, inds, vals)
     o = S.default_opts()
     o[0], o[3], o[1], o[4] = 1, 3, 0.0, 0
     csf = S.csf_alloc(dims, inds, vals, o)
     fit_ref, _, _ = restate.cpd_als(dims, inds, vals, 5, int(o[3]), float(o[1]), 2)      # rank 5 > dims[0] = 3: Gram of mode 0 singular
-    fit, lam, fac = S.cpd_als(csf.ptr, 5, o, seed=2)
-    assert np.isfinite(fit) and np.all(np.isfinite(lam))
-    assert abs(fit - fit_ref) < 1e-6
+    for host_solve in ("0", "1"):
+        monkeypatch.setenv("SPLATT_B200_HOST_SOLVE", host_solve)
+        fit, lam, fac = S.cpd_als(csf.ptr, 5, o, seed=2)
+        assert np.isfinite(fit) and np.all(np.isfinite(lam)), host_solve
+        assert abs(fit - fit_ref) < 1e-6, (host_solve, fit, fit_ref)
 
 
 @pytest.mark.parametrize("R", [8, 17, 32, 70])
