@@ -557,6 +557,49 @@ int splatt_b200_cpd_als_device_f32(splatt_b200_tensor const * t, int ncolumns, i
                                    double * lambda_out, double * fit_out, int * iterations_out,
                                    void * stream);
 
+/* Sum over the tensor's nonzeros of (v - sum_r lambda_r prod_m U_m[i_m, r])^2: the residual of a
+ * Kruskal model at the stored entries (e.g. a Tensor.cpd_als result scored on a held-out tensor).
+ *   d_factors[m]  dims[m] x ldm device matrices, row-major; columns [ncolumns, ldm) never feed
+ *                 the result (they may hold anything, NaN included).
+ *   lambda        ncolumns HOST doubles, or NULL for all ones.
+ * Works on any layout (it walks the tensor's first stream); a shard sums its own nonzeros.  Runs
+ * on t->device, enqueues on `stream` and synchronises it once.  Input rules: 1 <= ncolumns <= 64,
+ * ldm even and >= ncolumns, every d_factors[m] 16-byte aligned; otherwise SPLATT_ERROR_BADINPUT
+ * and nothing is enqueued. */
+int splatt_b200_tensor_sse(splatt_b200_tensor const * t, int ncolumns, int ldm,
+                           double const * const * d_factors, double const * lambda,
+                           double * sse_out, void * stream);
+
+/* Tensor completion by row-wise ALS: fits x^(i_1..i_N) = sum_r prod_m U_m[i_m, r] (no lambda) to
+ * the stored entries of `train` only (a coordinate that is not stored is unobserved, not zero;
+ * duplicate coordinates are separate observations), minimising
+ *     L = sum_{x stored} (v_x - x^_x)^2 + reg * sum_m ||U_m||_F^2,   reg = options[REGULARIZE].
+ * One iteration updates the modes 0 .. N-1 in order; row i of U_m becomes
+ *     (sum_x h_x h_x^T + reg I)^-1 sum_x v_x h_x   over the nonzeros x with mode-m index i,
+ * h_x the Hadamard product of the other modes' current rows (modes updated earlier in the same
+ * iteration with their new values).  A row with no observations becomes 0.
+ *   validate      may be NULL; else a tensor with train's nmodes and dims, on the same device,
+ *                 scored after every iteration.
+ *   d_factors[m]  dims[m] x ldm device matrices, in/out: the start on entry, the factors of the
+ *                 last iteration on return.  Columns [ncolumns, ldm) never feed the results and
+ *                 are never written.
+ *   history       NULL, or 3 doubles per iteration run: L, the training RMSE
+ *                 sqrt(sum (v - x^)^2 / nnz), and the validation RMSE (NaN without `validate`).
+ *   iterations_out the number of iterations run (may be NULL).
+ * Stops after options[NITER] iterations or, from the second iteration on, when
+ * |L_prev - L| / L_prev < options[TOLERANCE].  VERBOSITY above NONE prints one line per iteration.
+ * Runs on train->device, enqueues on `stream`, synchronises it once per iteration (the history).
+ * Input rules: 1 <= ncolumns <= 64; ldm even and >= ncolumns; every d_factors[m] 16-byte aligned;
+ * reg finite and > 0; both tensors whole (shard_count <= 1); train built with the ALLROOT layout
+ * (every mode served by a root stream; ASGIVEN is rejected).  Leaf-tiled streams (CTA-tiled by
+ * default, or ktile > 0) are accepted.  A violation returns SPLATT_ERROR_BADINPUT before anything is
+ * enqueued, and the factors are left untouched. */
+int splatt_b200_tc_als_device(splatt_b200_tensor const * train,
+                              splatt_b200_tensor const * validate,
+                              int ncolumns, int ldm, double const * options,
+                              double * const * d_factors, double * history,
+                              int * iterations_out, void * stream);
+
 /* Measurement aid: a pure gather kernel with the MTTKRP's access pattern (whole
  * fp64 rows of a rows x ldm matrix at d_idx[0..nidx), 128-bit loads, eight rows in
  * flight per lane group, no arithmetic).  bench.py times it to report a MEASURED

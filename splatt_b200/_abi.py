@@ -103,7 +103,7 @@ EXPORTS = [
     "splatt_b200_als_tail_gram_f32", "splatt_b200_als_tail_update_f32",
     "splatt_b200_als_tail_fit_f32", "splatt_b200_cpd_als_device", "splatt_b200_cpd_als_device_f32",
     "splatt_b200_tensor_shard", "splatt_b200_mttkrp_multicast_sync",
-    "splatt_b200_mttkrp_multicast_sync_columns",
+    "splatt_b200_mttkrp_multicast_sync_columns", "splatt_b200_tensor_sse", "splatt_b200_tc_als_device",
     "splatt_b200_multi_env_devices", "splatt_b200_multi_create", "splatt_b200_multi_free",
     "splatt_b200_multi_info", "splatt_b200_multi_mttkrp_host", "splatt_b200_multi_cpd_als",
     "splatt_b200_multi_last_ms", "splatt_b200_build_count", "splatt_b200_cache_clear",
@@ -206,6 +206,13 @@ def load() -> C.CDLL:
                                                    C.POINTER(C.c_double), C.POINTER(f32_p), val_p,
                                                    C.POINTER(C.c_double), C.POINTER(C.c_int),
                                                    C.c_void_p]
+    lib.splatt_b200_tensor_sse.restype = C.c_int
+    lib.splatt_b200_tensor_sse.argtypes = [C.c_void_p, C.c_int, C.c_int, vpp, val_p,
+                                           C.POINTER(C.c_double), C.c_void_p]
+    lib.splatt_b200_tc_als_device.restype = C.c_int
+    lib.splatt_b200_tc_als_device.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int,
+                                              C.POINTER(C.c_double), vpp, val_p,
+                                              C.POINTER(C.c_int), C.c_void_p]
     lib.splatt_b200_csf_to_coo.restype = C.c_int
     lib.splatt_b200_csf_to_coo.argtypes = [csf_p, u32pp, val_p]
     lib.splatt_b200_gather_probe.restype = C.c_int

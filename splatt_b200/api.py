@@ -394,6 +394,97 @@ class Tensor:
         _check(rc, sym)
         return fit.value, lam, [b[:, :rank] for b in bufs], its.value
 
+    def sse(self, factors, lam=None, stream=None) -> float:
+        """Sum over this tensor's nonzeros of (v - sum_r lam_r prod_m factors[m][i_m, r])^2
+        (splatt_b200_tensor_sse; lam None = all ones).  factors: float64 CUDA tensors
+        (dims[m] x rank) on the current device; rank <= 64.  Synchronises the stream once."""
+        import torch
+        dev = torch.device("cuda", torch.cuda.current_device())
+        if len(factors) != self.nmodes:
+            raise ValueError(f"{len(factors)} factor matrices for a {self.nmodes}-mode tensor")
+        rank = factors[0].shape[1] if factors[0].dim() == 2 else -1
+        for m, f in enumerate(factors):
+            if f.dtype != torch.float64:
+                raise ValueError(f"factor matrix {m} is {f.dtype}; Tensor.sse is float64 only")
+            if f.device != dev or tuple(f.shape) != (self.dims[m], rank):
+                raise ValueError(f"factor matrix {m} must be a tensor of shape "
+                                 f"({self.dims[m]}, {rank}) on the current device {dev}")
+        ldm = rank + (rank & 1)
+        bufs = [torch.zeros((d, ldm), dtype=torch.float64, device=dev) for d in self.dims]
+        for b, f in zip(bufs, factors):
+            b[:, :rank].copy_(f)
+        lam_a = None if lam is None else np.ascontiguousarray(lam, dtype=np.float64)
+        if lam_a is not None and lam_a.shape != (rank,):
+            raise ValueError(f"lam must have {rank} entries")
+        if stream is None:
+            s = torch.cuda.current_stream(dev).cuda_stream
+        else:
+            torch.cuda.current_stream(dev).synchronize()    # the buffers were filled there
+            s = stream
+        ptrs = (A.val_p * self.nmodes)(*[C.cast(C.c_void_p(b.data_ptr()), A.val_p) for b in bufs])
+        out = C.c_double()
+        rc = self.lib.splatt_b200_tensor_sse(self.h, rank, ldm, ptrs,
+                                             A.val_p() if lam_a is None else _dptr(lam_a),
+                                             C.byref(out), C.c_void_p(s))
+        _check(rc, "splatt_b200_tensor_sse")
+        return out.value
+
+    def complete(self, rank: int, factors=None, *, validate: Optional["Tensor"] = None, reg: float,
+                 niters: int = 50, tol: float = 1e-4, seed: int = 0, verbosity: int = 0,
+                 stream=None):
+        """Tensor completion by row-wise ALS (splatt_b200_tc_als_device): fits
+        sum_r prod_m U_m[i_m, r] to this tensor's stored entries only, with the penalty
+        reg * sum_m ||U_m||_F^2 (reg > 0).  Needs a whole tensor built with the ALLROOT layout
+        on the current CUDA device, and 1 <= rank <= 64.  float64 only.
+
+        factors: list of float64 CUDA tensors (dims[m] x rank), the start; copied into padded
+        buffers, never written.  None: uniform on [0, 1) from a torch.Generator on the current
+        device seeded with `seed`, drawn mode by mode.  validate: a Tensor with the same shape,
+        scored after every iteration.  Stops after `niters` iterations or, from the second on,
+        when the objective moved by less than `tol` relative.
+        Returns (history: numpy float64 [iterations x 3] of (objective, training RMSE,
+        validation RMSE or NaN), factors (CUDA views dims[m] x rank), iterations)."""
+        import torch
+        dev = torch.device("cuda", torch.cuda.current_device())
+        if factors is not None:
+            if len(factors) != self.nmodes:
+                raise ValueError(f"{len(factors)} factor matrices for a {self.nmodes}-mode tensor")
+            for m, f in enumerate(factors):
+                if f.dtype != torch.float64:
+                    raise ValueError(f"factor matrix {m} is {f.dtype}; completion is float64 only")
+                if f.device != dev or tuple(f.shape) != (self.dims[m], rank):
+                    raise ValueError(f"factor matrix {m} must be a tensor of shape "
+                                     f"({self.dims[m]}, {rank}) on the current device {dev}")
+        if validate is not None and not isinstance(validate, Tensor):
+            raise ValueError("validate must be a Tensor")
+        ldm = rank + (rank & 1)
+        bufs = [torch.zeros((d, ldm), dtype=torch.float64, device=dev) for d in self.dims]
+        if factors is None:
+            g = torch.Generator(device=dev).manual_seed(seed)
+            for b in bufs:
+                b[:, :rank].uniform_(0.0, 1.0, generator=g)
+        else:
+            for b, f in zip(bufs, factors):
+                b[:, :rank].copy_(f)
+        o = default_opts()
+        o[A.OPTION_NITER] = niters
+        o[A.OPTION_TOLERANCE] = tol
+        o[A.OPTION_VERBOSITY] = verbosity
+        o[A.OPTION_REGULARIZE] = reg
+        if stream is None:
+            s = torch.cuda.current_stream(dev).cuda_stream
+        else:
+            torch.cuda.current_stream(dev).synchronize()    # the buffers were filled there
+            s = stream
+        ptrs = (A.val_p * self.nmodes)(*[C.cast(C.c_void_p(b.data_ptr()), A.val_p) for b in bufs])
+        hist = np.full((max(int(niters), 0), 3), np.nan)
+        its = C.c_int()
+        rc = self.lib.splatt_b200_tc_als_device(self.h, None if validate is None else validate.h,
+                                                rank, ldm, _dptr(o), ptrs, _dptr(hist),
+                                                C.byref(its), C.c_void_p(s))
+        _check(rc, "splatt_b200_tc_als_device")
+        return hist[:its.value].copy(), [b[:, :rank] for b in bufs], its.value
+
     def shard(self, rank: int, count: int, device: int = -1) -> "Tensor":
         """Cut shard `rank` of `count` out of this (whole) tensor onto `device`
         (splatt_b200_tensor_shard): the equal-nnz chunk range of every stream, copied

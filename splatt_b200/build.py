@@ -32,7 +32,7 @@ def _units():
         units.append((f"mttkrp_inst_n{n}", CSRC / "mttkrp_inst.cu", [f"-DSPB200_INST_N={n}"]))
         units.append((f"mttkrp_inst_f32_n{n}", CSRC / "mttkrp_inst.cu",
                       [f"-DSPB200_INST_N={n}", "-DSPB200_INST_F32"]))
-    for name in ("mttkrp_launch", "mttkrp_tiled", "stream_build", "engine", "dropin", "cpd", "multi"):
+    for name in ("mttkrp_launch", "mttkrp_tiled", "stream_build", "engine", "dropin", "cpd", "multi", "tc"):
         units.append((name, CSRC / f"{name}.cu", []))
     return units
 
