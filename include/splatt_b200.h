@@ -650,6 +650,76 @@ int splatt_b200_cp_apr_device(splatt_b200_tensor const * t, int ncolumns, int ld
                               double * const * d_factors, double * lambda_out,
                               double * history, int * iterations_out, void * stream);
 
+/* TTMc, the kernel of Tucker: d_out = X_(mode) (kron_{m != mode} U_m), a dims[mode] x C_mode
+ * row-major device matrix with leading dimension C_mode = prod_{m != mode} ranks[m], U_m =
+ * columns [0, ranks[m]) of d_mats[m] (dims[m] x ldm, row-major).  Column order: the other modes
+ * in increasing mode order, the highest fastest (c = sum_{m != mode} j_m prod_{m' > m, m' != mode}
+ * ranks[m']), whatever the stream's level order.  Unstored coordinates are zeros; duplicate
+ * coordinates add.  d_out is zeroed, then written.  d_mats[mode] is not read (may be NULL).
+ * Runs on t->device and enqueues on `stream` (boundary-slot scratch is allocated and freed
+ * stream-ordered); no host synchronisation.  On untiled streams the result is bitwise
+ * reproducible; on leaf-tiled streams (CTA-tiled or ktile > 0) pieces of a row are added with
+ * atomics and may vary in the last bits.
+ * Input rules: the tensor whole (shard_count <= 1) and built with the ALLROOT layout; 2 <= N <= 8;
+ * 0 <= mode < N; 1 <= ranks[m] <= min(32, dims[m]) for every m; C_mode <= 1024; ldm even and
+ * >= every ranks[m]; d_out and every d_mats[m], m != mode, 16-byte aligned.  A violation returns
+ * SPLATT_ERROR_BADINPUT and nothing is enqueued. */
+int splatt_b200_ttmc(splatt_b200_tensor const * t, int mode, int const * ranks, int ldm,
+                     double const * const * d_mats, double * d_out, void * stream);
+
+/* Parameters of HOOI's subspace step beyond options[NITER] and options[TOLERANCE]. */
+typedef struct {
+  int    max_power;      /* orthogonal-iteration steps per mode and iteration, >= 1 (default 50) */
+  double svd_tol;        /* stop the steps when the subspace moved by <= this, >= 0 (default 1e-10) */
+} splatt_b200_tucker_opts;
+
+/* Sparse Tucker decomposition by HOOI (higher-order orthogonal iteration):
+ *     X ~ G x_0 U_0 x_1 U_1 ... x_{N-1} U_{N-1},
+ * U_m dims[m] x ranks[m] with orthonormal columns, G the ranks[0] x ... x ranks[N-1] core.
+ * Unstored coordinates are zeros; duplicate coordinates add (in the TTMc and in ||X||^2).
+ * Start: columns [0, ranks[m]) of d_factors[m], each orthonormalised by CholeskyQR2 in fp64.
+ * One iteration runs, for n = 0 .. N-1 (modes updated earlier in the iteration with their new
+ * values):
+ *   1. Y_n = splatt_b200_ttmc(n), dims[n] x C_n;
+ *   2. from Q = U_n, up to max_power steps of Q <- orth(Y_n Y_n^T Q + mu Q), orth = CholeskyQR2,
+ *      mu = 2^-20 ||Y_n||_F^2 (1 when Y_n = 0): the shift keeps CholeskyQR well posed when Y_n
+ *      has rank below R_n and leaves the eigenvectors unchanged; the steps stop early once
+ *      ||Q_new - Q_old (Q_old^T Q_new)||_F <= svd_tol;
+ *   3. Rayleigh-Ritz: W = Y_n^T Q, W^T W = V diag(lam) V^T (Jacobi, lam descending),
+ *      U_n = Q V; in every column the entry of largest magnitude is made positive (the lowest
+ *      row on a tie).
+ * After the last mode G = (W V with U_{N-1}'s column signs), whose C_{N-1} x R_{N-1} row-major
+ * array is the C-order array of shape (ranks[0], ..., ranks[N-1]), and
+ *     fit = 1 - sqrt(max(||X||^2 - ||G||_F^2, 0)) / ||X||.
+ * Stops after options[NITER] iterations, or when fit = 1, or from the second iteration on when
+ * |fit - previous fit| < options[TOLERANCE].  VERBOSITY above NONE prints one line per
+ * iteration.  A rank-deficient Y_n still gives orthonormal U_n (the columns past its rank are
+ * some orthonormal completion, with zero core entries).
+ *   topts         NULL for the defaults (50, 1e-10).
+ *   d_factors[m]  dims[m] x ldm device matrices, in/out: the start on entry, the factors of the
+ *                 last iteration on return (the orthonormalised start when NITER = 0).  Columns
+ *                 [ranks[m], ldm) never feed a result and are never written.
+ *   core_out      prod ranks[m] HOST doubles, the core of the last iteration (untouched when no
+ *                 iteration ran).
+ *   history       NULL, or 4 doubles per iteration run: the fit, ||G||_F, the orthogonal-
+ *                 iteration steps summed over the modes, and the largest final subspace residual.
+ *   iterations_out the number of iterations run (may be NULL).
+ * The factors are only written on success.  On untiled streams the factors, the core and the
+ * history are bitwise reproducible from run to run (every reduction has a fixed order); on
+ * leaf-tiled streams the TTMc adds with atomics.  Runs on t->device, enqueues on `stream` and
+ * synchronises it once per orthogonal-iteration step (the residual), once per mode (the R x R
+ * Ritz matrix, diagonalised on the host) and once per iteration (the fit and the core).
+ * Input rules: the tensor whole and ALLROOT (leaf-tiled streams accepted); 2 <= N <= 8;
+ * 1 <= ranks[m] <= min(32, dims[m]); ranks[n] <= C_n <= 1024 for every n; ldm even and >= every
+ * ranks[m]; every d_factors[m] 16-byte aligned; max_power >= 1; svd_tol, TOLERANCE >= 0 and
+ * finite; 0 <= NITER < 2^31; every start factor with independent columns (a Gram pivot above
+ * 2^-46 of its diagonal entry in CholeskyQR).  A violation returns SPLATT_ERROR_BADINPUT and the
+ * factors are left bit-identical. */
+int splatt_b200_tucker_hooi_device(splatt_b200_tensor const * t, int const * ranks, int ldm,
+                                   double const * options, splatt_b200_tucker_opts const * topts,
+                                   double * const * d_factors, double * core_out,
+                                   double * history, int * iterations_out, void * stream);
+
 /* Measurement aid: a pure gather kernel with the MTTKRP's access pattern (whole
  * fp64 rows of a rows x ldm matrix at d_idx[0..nidx), 128-bit loads, eight rows in
  * flight per lane group, no arithmetic).  bench.py times it to report a MEASURED

@@ -543,6 +543,107 @@ class Tensor:
         _check(rc, "splatt_b200_cp_apr_device")
         return lam, [b[:, :rank] for b in bufs], hist[:its.value].copy(), its.value
 
+    def ttmc(self, mode: int, mats, out, ranks):
+        """TTMc (splatt_b200_ttmc): out = X_(mode) times the Kronecker product of mats[m][:, :ranks[m]],
+        m != mode, columns in mode order with the highest mode fastest.  mats: float64 CUDA tensors
+        (dims[m] x >= ranks[m]; mats[mode] may be None); out: a contiguous float64 CUDA tensor of
+        shape (dims[mode], prod_{m != mode} ranks[m]).  Needs a whole ALLROOT tensor on the current
+        device, 1 <= ranks[m] <= min(32, dims[m]) and at most 1024 columns.  Enqueued on the current
+        stream; returns out."""
+        import torch
+        dev = torch.device("cuda", torch.cuda.current_device())
+        ranks = [int(r) for r in ranks]
+        if len(mats) != self.nmodes or len(ranks) != self.nmodes:
+            raise ValueError(f"need {self.nmodes} matrices and ranks")
+        C_ = int(np.prod([r for m, r in enumerate(ranks) if m != mode]))
+        if (out.dtype != torch.float64 or out.device != dev or not out.is_contiguous() or
+                tuple(out.shape) != (self.dims[mode], C_)):
+            raise ValueError(f"out must be a contiguous float64 tensor of shape ({self.dims[mode]}, {C_}) "
+                             f"on {dev}")
+        ldm = max(ranks) + (max(ranks) & 1)
+        bufs = []
+        for m, f in enumerate(mats):
+            if m == mode:
+                bufs.append(None)
+                continue
+            if f.dtype != torch.float64 or f.device != dev or f.dim() != 2 or f.shape[0] != self.dims[m] \
+                    or f.shape[1] < ranks[m]:
+                raise ValueError(f"matrix {m} must be a float64 tensor of shape ({self.dims[m]}, >= "
+                                 f"{ranks[m]}) on {dev}")
+            b = torch.zeros((self.dims[m], ldm), dtype=torch.float64, device=dev)
+            b[:, :ranks[m]].copy_(f[:, :ranks[m]])
+            bufs.append(b)
+        ptrs = (A.val_p * self.nmodes)(*[A.val_p() if b is None else C.cast(C.c_void_p(b.data_ptr()), A.val_p)
+                                         for b in bufs])
+        rk = (C.c_int * self.nmodes)(*ranks)
+        s = torch.cuda.current_stream(dev).cuda_stream
+        rc = self.lib.splatt_b200_ttmc(self.h, mode, rk, ldm, ptrs,
+                                       C.cast(C.c_void_p(out.data_ptr()), A.val_p), C.c_void_p(s))
+        _check(rc, "splatt_b200_ttmc")
+        torch.cuda.current_stream(dev).synchronize()     # the padded copies must outlive the kernel
+        return out
+
+    def tucker(self, ranks, factors=None, *, niters: int = 50, tol: float = 1e-5, max_power: int = 50,
+               svd_tol: float = 1e-10, seed: int = 0, verbosity: int = 0, stream=None):
+        """Sparse Tucker decomposition by HOOI (splatt_b200_tucker_hooi_device):
+        X ~ core x_0 U_0 ... x_{N-1} U_{N-1} with orthonormal factors U_m (dims[m] x ranks[m]).
+        Needs a whole ALLROOT tensor on the current CUDA device, 1 <= ranks[m] <= min(32, dims[m])
+        and ranks[n] <= prod_{m != n} ranks[m] <= 1024.  float64 only.
+
+        factors: list of float64 CUDA tensors (dims[m] x ranks[m]), the start (orthonormalised by
+        the call; its columns must be independent); copied into padded buffers, never written.
+        None: standard normal from a torch.Generator on the current device seeded with `seed`,
+        drawn mode by mode.  Each mode runs at most `max_power` orthogonal-iteration steps and
+        stops them when the subspace moved by <= svd_tol; the run stops after `niters`
+        iterations or when the fit moved by less than `tol`.
+        Returns (core (numpy float64 of shape ranks), factors (CUDA views dims[m] x ranks[m]),
+        history (numpy float64 [iterations x 4] of (fit, ||core||_F, orthogonal-iteration steps
+        summed over the modes, largest final subspace residual)), iterations)."""
+        import torch
+        dev = torch.device("cuda", torch.cuda.current_device())
+        ranks = [int(r) for r in ranks]
+        if len(ranks) != self.nmodes:
+            raise ValueError(f"{len(ranks)} ranks for a {self.nmodes}-mode tensor")
+        if factors is not None:
+            if len(factors) != self.nmodes:
+                raise ValueError(f"{len(factors)} factor matrices for a {self.nmodes}-mode tensor")
+            for m, f in enumerate(factors):
+                if f.dtype != torch.float64:
+                    raise ValueError(f"factor matrix {m} is {f.dtype}; Tucker is float64 only")
+                if f.device != dev or tuple(f.shape) != (self.dims[m], ranks[m]):
+                    raise ValueError(f"factor matrix {m} must be a tensor of shape "
+                                     f"({self.dims[m]}, {ranks[m]}) on the current device {dev}")
+        ldm = max(ranks) + (max(ranks) & 1)
+        bufs = [torch.zeros((d, ldm), dtype=torch.float64, device=dev) for d in self.dims]
+        if factors is None:
+            g = torch.Generator(device=dev).manual_seed(seed)
+            for b, r in zip(bufs, ranks):
+                b[:, :r].normal_(0.0, 1.0, generator=g)
+        else:
+            for b, f, r in zip(bufs, factors, ranks):
+                b[:, :r].copy_(f)
+        o = default_opts()
+        o[A.OPTION_NITER] = niters
+        o[A.OPTION_TOLERANCE] = tol
+        o[A.OPTION_VERBOSITY] = verbosity
+        to = A.TuckerOpts(max_power, svd_tol)
+        if stream is None:
+            s = torch.cuda.current_stream(dev).cuda_stream
+        else:
+            torch.cuda.current_stream(dev).synchronize()    # the buffers were filled there
+            s = stream
+        ptrs = (A.val_p * self.nmodes)(*[C.cast(C.c_void_p(b.data_ptr()), A.val_p) for b in bufs])
+        rk = (C.c_int * self.nmodes)(*ranks)
+        core = np.zeros(int(np.prod(ranks)))
+        hist = np.full((max(int(niters), 0), 4), np.nan)
+        its = C.c_int()
+        rc = self.lib.splatt_b200_tucker_hooi_device(self.h, rk, ldm, _dptr(o), C.byref(to), ptrs,
+                                                     _dptr(core), _dptr(hist), C.byref(its),
+                                                     C.c_void_p(s))
+        _check(rc, "splatt_b200_tucker_hooi_device")
+        return (core.reshape(ranks), [b[:, :r] for b, r in zip(bufs, ranks)], hist[:its.value].copy(),
+                its.value)
+
     def shard(self, rank: int, count: int, device: int = -1) -> "Tensor":
         """Cut shard `rank` of `count` out of this (whole) tensor onto `device`
         (splatt_b200_tensor_shard): the equal-nnz chunk range of every stream, copied

@@ -1,7 +1,8 @@
-// The per-record walk of a root stream that completion (tc.cu) and Poisson CP (apr.cu) share:
-// one warp per nnz-balanced chunk range of the root MTTKRP, a private TMA record ring, the
-// Hadamard prefix of the inner levels in registers.  Also the model-sum kernel body (the SSE of
-// completion, the log-likelihood of CP-APR) and the host helpers both drivers use.
+// The per-record walk of a root stream that completion (tc.cu), Poisson CP (apr.cu) and Tucker
+// (tucker.cu) share: one warp per nnz-balanced chunk range of the root MTTKRP, a private TMA
+// record ring, and for completion and CP-APR the Hadamard prefix of the inner levels in registers.
+// Also the model-sum kernel body (the SSE of completion, the log-likelihood of CP-APR) and the
+// host helpers the drivers use.
 #pragma once
 #include "mttkrp_kernels.cuh"
 #include <algorithm>
@@ -128,6 +129,91 @@ __device__ __forceinline__ void walk_range(const TcArgs & a, unsigned char * sme
         else row = __ldg(&a.up[0][pos[0]]);
       }
       f(v, h, close, row, off + n + 1 == T);
+      if (c) {
+#pragma unroll
+        for (int l = 0; l <= N - 3; ++l)
+          if (c >= uint32_t(N - 1 - l)) ++pos[l];
+      }
+      pc = c;
+    }
+    __syncwarp();
+    if (step + kStages < steps) issue(step + kStages);
+  }
+}
+
+// The same walk without the Hadamard prefix, for kernels that need the level structure itself
+// (Tucker's TTMc forms a Kronecker product of the levels' rows).  For every record
+// g(q, pc, pos, close, row, last) is called by the whole warp: q = the record, pc = the previous
+// record's close count (levels N-1-pc .. N-2 have a new node at this record; pc = N-1 at the
+// range's first record), pos[l] = the node number of level l = 0 .. N-3 (its index is
+// up[l][pos[l]]; level N-2's is the record's parent field), close / row / last as in walk_range
+// (row valid when close).  walk_range keeps its own copy of this loop: rebasing it on walk_levels
+// reschedules the SASS of the completion and CP-APR kernels.
+template <int N, class G>
+__device__ __forceinline__ void walk_levels(const TcArgs & a, unsigned char * smem, G && g) {
+  constexpr int SU   = kStageRecs;
+  const int     warp = threadIdx.x >> 5;
+  const int     lane = threadIdx.x & 31;
+  SpRec *    ring = reinterpret_cast<SpRec *>(smem) + warp * kStages * SU;
+  uint64_t * bars = reinterpret_cast<uint64_t *>(smem + smem_rec_bytes(kStages, 1, 0)) + warp * kStages;
+  if (lane == 0) {
+#pragma unroll
+    for (int s = 0; s < kStages; ++s) mbar_init(&bars[s], 1);
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+  }
+  __syncwarp();
+
+  const unsigned long long TG = static_cast<unsigned long long>(gridDim.x) * kWarps;
+  const unsigned long long gg = static_cast<unsigned long long>(blockIdx.x) * kWarps + warp;
+  const unsigned long long cb = gg * a.nchunks / TG;
+  const unsigned long long ce = (gg + 1) * a.nchunks / TG;
+  const unsigned long long rb = cb * SPB200_CHUNK;
+  unsigned long long       re = ce * SPB200_CHUNK;
+  if (re > a.nrec) re = a.nrec;
+  const uint32_t T     = (re > rb) ? static_cast<uint32_t>(re - rb) : 0u;
+  const uint32_t steps = (T + SU - 1) / SU;
+
+  auto issue = [&](uint32_t step) {
+    if (lane != 0) return;
+    uint64_t *     bar = &bars[step % kStages];
+    const uint32_t off = step * SU;
+    const uint32_t cnt = min(static_cast<uint32_t>(SU), T - off);
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    mbar_arrive_expect_tx(bar, cnt * 16u);
+    tma_bulk_g2s(&ring[(step % kStages) * SU], a.rec + rb + off, cnt * 16u, bar);
+  };
+
+  constexpr int NP = (N > 2) ? N - 2 : 1;
+  uint32_t      pos[NP];
+#pragma unroll
+  for (int l = 0; l < NP; ++l) pos[l] = 0u;
+#pragma unroll
+  for (int l = 0; l < N - 2; ++l) pos[l] = T ? a.desc[cb * (N - 2) + l] : 0u;
+  uint32_t pc = N - 1;
+
+#pragma unroll
+  for (int s = 0; s < kStages; ++s)
+    if (s < static_cast<int>(steps)) issue(s);
+
+  for (uint32_t step = 0; step < steps; ++step) {
+    while (!mbar_try_wait(&bars[step % kStages], (step / kStages) & 1u)) {}
+    const uint32_t off = step * SU;
+    const uint32_t cnt = min(static_cast<uint32_t>(SU), T - off);
+    SpRec *        buf = &ring[(step % kStages) * SU];
+    if (lane == 0 && off + cnt == T)
+      buf[cnt - 1].aux = (buf[cnt - 1].aux & SPB200_IDX_MASK) | (uint32_t(N - 1) << SPB200_IDX_BITS);
+    __syncwarp();
+    for (uint32_t n = 0; n < cnt; ++n) {
+      const uint4    q     = *reinterpret_cast<const uint4 *>(&buf[n]);
+      const uint32_t c     = q.w >> SPB200_IDX_BITS;
+      const bool     close = c >= uint32_t(N - 1);
+      uint32_t       row   = 0;
+      if (close) {
+        if constexpr (N == 2) row = q.w & SPB200_IDX_MASK;
+        else row = __ldg(&a.up[0][pos[0]]);
+      }
+      g(q, pc, pos, close, row, off + n + 1 == T);
       if (c) {
 #pragma unroll
         for (int l = 0; l <= N - 3; ++l)
