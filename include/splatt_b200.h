@@ -557,6 +557,49 @@ int splatt_b200_cpd_als_device_f32(splatt_b200_tensor const * t, int ncolumns, i
                                    double * lambda_out, double * fit_out, int * iterations_out,
                                    void * stream);
 
+/* Nonnegative CPD of a device-resident tensor by HALS (hierarchical ALS: Cichocki & Phan 2009,
+ * Gillis & Glineur 2012).  The model is K = sum_r lambda_r a_r^(0) o ... o a_r^(N-1) with
+ * nonnegative factors whose columns have 2-norm 1 and lambda >= 0; the call minimises
+ * 1/2 ||X - K||^2 over the stored entries, unstored entries read as zeros (as CPD-ALS does).
+ * Tensor values may have any sign: the constraint is on the factors.
+ *   Start: the caller's factors, columns [0, ncolumns).  Every column is 2-normalised and lambda
+ *     is the product of the norms; then the Grams are formed.
+ *   One iteration, for n = 0 .. N-1:
+ *     M = the MTTKRP of mode n;  G = the Hadamard product of the other modes' Grams;
+ *     B = A_n diag(lambda);  one Gauss-Seidel sweep over the columns r = 0 .. R-1,
+ *       B[:, r] <- max(eps, (M[:, r] - sum_{j != r} B[:, j] G[j, r]) / G[r, r])
+ *     (columns j < r already hold their new values);  lambda = the column 2-norms of B,
+ *     A_n = B diag(1 / lambda) (always the 2-norm), and the Gram of A_n.
+ *   The floor eps = 1e-16 is applied in fp64.  It keeps every column nonzero, so after the
+ *   normalisation every G[r, r] is 1 up to rounding.  The division by G[r, r] is computed as a
+ *   product with its reciprocal.
+ * Fit, stopping and verbosity are those of splatt_b200_cpd_als_device: the fit
+ * 1 - sqrt(||X||^2 + ||K||^2 - 2<X,K>) / ||X|| is formed from the last mode's M, and the run stops
+ * after NITER iterations, at fit == 1, or when the fit moved by less than TOLERANCE (from the
+ * second iteration on).
+ *   d_factors[m]  in/out: the start on entry; on return the loop's factors as they stand (already
+ *                 2-normalised, no post-processing).  Columns [ncolumns, ldm) are never written
+ *                 and never feed the results.
+ *   lambda_out, fit_out, iterations_out: as for splatt_b200_cpd_als_device (each may be NULL).
+ *   history       NULL, or room for NITER doubles: the fit of every iteration run.
+ * Input rules: those of splatt_b200_cpd_als_device; in addition every start entry in columns
+ * [0, ncolumns) must be finite and >= 0, and every start column must have a positive, finite sum
+ * of squares (so a nonzero entry; the sums are formed in fp64).  The start is checked on the
+ * device before anything is written; a violation returns SPLATT_ERROR_BADINPUT and leaves the
+ * factors bit-identical.  Synchronises the stream as splatt_b200_cpd_als_device does, and once
+ * more for the start check.
+ * _f32: fp32 factors and MTTKRP (splatt_b200_mttkrp_f32); G, the sweep's arithmetic, lambda and the
+ * fit are fp64, and each swept row is rounded to fp32 once.  The fp32 fit resolves only about
+ * 1e-4 near 1, as described for splatt_b200_cpd_als_device_f32. */
+int splatt_b200_cpd_nonneg_device(splatt_b200_tensor const * t, int ncolumns, int ldm,
+                                  double const * options, double * const * d_factors,
+                                  double * lambda_out, double * fit_out, int * iterations_out,
+                                  double * history, void * stream);
+int splatt_b200_cpd_nonneg_device_f32(splatt_b200_tensor const * t, int ncolumns, int ldm,
+                                      double const * options, float * const * d_factors,
+                                      double * lambda_out, double * fit_out, int * iterations_out,
+                                      double * history, void * stream);
+
 /* Sum over the tensor's nonzeros of (v - sum_r lambda_r prod_m U_m[i_m, r])^2: the residual of a
  * Kruskal model at the stored entries (e.g. a Tensor.cpd_als result scored on a held-out tensor).
  *   d_factors[m]  dims[m] x ldm device matrices, row-major; columns [ncolumns, ldm) never feed

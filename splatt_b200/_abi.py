@@ -111,6 +111,7 @@ EXPORTS = [
     "splatt_b200_als_tail_update", "splatt_b200_als_tail_fit", "splatt_b200_csf_to_coo",
     "splatt_b200_als_tail_gram_f32", "splatt_b200_als_tail_update_f32",
     "splatt_b200_als_tail_fit_f32", "splatt_b200_cpd_als_device", "splatt_b200_cpd_als_device_f32",
+    "splatt_b200_cpd_nonneg_device", "splatt_b200_cpd_nonneg_device_f32",
     "splatt_b200_tensor_shard", "splatt_b200_mttkrp_multicast_sync",
     "splatt_b200_mttkrp_multicast_sync_columns", "splatt_b200_tensor_sse", "splatt_b200_tc_als_device",
     "splatt_b200_cp_apr_device", "splatt_b200_ttmc", "splatt_b200_tucker_hooi_device",
@@ -216,6 +217,16 @@ def load() -> C.CDLL:
                                                    C.POINTER(C.c_double), C.POINTER(f32_p), val_p,
                                                    C.POINTER(C.c_double), C.POINTER(C.c_int),
                                                    C.c_void_p]
+    lib.splatt_b200_cpd_nonneg_device.restype = C.c_int
+    lib.splatt_b200_cpd_nonneg_device.argtypes = [C.c_void_p, C.c_int, C.c_int,
+                                                  C.POINTER(C.c_double), vpp, val_p,
+                                                  C.POINTER(C.c_double), C.POINTER(C.c_int), val_p,
+                                                  C.c_void_p]
+    lib.splatt_b200_cpd_nonneg_device_f32.restype = C.c_int
+    lib.splatt_b200_cpd_nonneg_device_f32.argtypes = [C.c_void_p, C.c_int, C.c_int,
+                                                      C.POINTER(C.c_double), C.POINTER(f32_p), val_p,
+                                                      C.POINTER(C.c_double), C.POINTER(C.c_int),
+                                                      val_p, C.c_void_p]
     lib.splatt_b200_tensor_sse.restype = C.c_int
     lib.splatt_b200_tensor_sse.argtypes = [C.c_void_p, C.c_int, C.c_int, vpp, val_p,
                                            C.POINTER(C.c_double), C.c_void_p]

@@ -344,6 +344,28 @@ class Tensor:
         the run before `niters` there.
         Returns (fit, lambda (numpy float64[rank]), factors (2-normalised, CUDA views
         dims[m] x rank), iterations)."""
+        fit, lam, facs, its, _ = self._cpd_device(False, rank, factors, dtype, niters, tol, seed,
+                                                  verbosity, stream)
+        return fit, lam, facs, its
+
+    def cpd_nonneg(self, rank: int, factors=None, *, dtype=None, niters: int = 50,
+                   tol: float = 1e-5, seed: int = 0, verbosity: int = 0, stream=None):
+        """Nonnegative CPD by HALS (splatt_b200_cpd_nonneg_device, or _f32 for float32: fp32
+        factors and MTTKRP, fp64 Hadamard Grams, sweep, lambda and fit) of this (whole) tensor on
+        its device: nonnegative factors with unit 2-norm columns and lambda >= 0 that minimise
+        1/2 ||X - K||^2, unstored entries read as zeros.  Tensor values may have any sign.  One
+        Gauss-Seidel sweep over the columns per mode and iteration, with every entry floored at
+        1e-16 (see include/splatt_b200.h).  The tensor must live on the current CUDA device.
+
+        factors: list of CUDA tensors (dims[m] x rank) of one dtype, the start (finite, >= 0, no
+        zero column); copied into padded buffers, never written.  None: uniform on [0, 1) from a
+        torch.Generator seeded with `seed`, in `dtype` (default float64).  Stops as cpd_als does.
+        Returns (fit, lambda (numpy float64[rank]), factors (CUDA views dims[m] x rank),
+        iterations, history (numpy float64[iterations]: the fit of every iteration))."""
+        return self._cpd_device(True, rank, factors, dtype, niters, tol, seed, verbosity, stream)
+
+    def _cpd_device(self, nonneg, rank, factors, dtype, niters, tol, seed, verbosity, stream):
+        """cpd_als (nonneg False) or cpd_nonneg: (fit, lambda, factors, iterations, history)."""
         import torch
         if factors is not None:
             dt = factors[0].dtype
@@ -371,8 +393,9 @@ class Tensor:
         bufs = [torch.zeros((d, ldm), dtype=dt, device=dev) for d in self.dims]
         if factors is None:
             g = torch.Generator(device=dev).manual_seed(seed)
+            lo, hi = (0.0, 1.0) if nonneg else (-3.0, 3.0)
             for b in bufs:
-                b[:, :rank].uniform_(-3.0, 3.0, generator=g)
+                b[:, :rank].uniform_(lo, hi, generator=g)
         else:
             for b, f in zip(bufs, factors):
                 b[:, :rank].copy_(f)
@@ -389,10 +412,18 @@ class Tensor:
         lam = np.zeros(rank)
         fit = C.c_double()
         its = C.c_int()
-        rc = getattr(self.lib, sym)(self.h, rank, ldm, _dptr(o), ptrs, _dptr(lam), C.byref(fit),
-                                    C.byref(its), C.c_void_p(s))
+        if nonneg:
+            sym = sym.replace("_als_", "_nonneg_")
+            hist = np.full(max(int(niters), 0), np.nan)
+            rc = getattr(self.lib, sym)(self.h, rank, ldm, _dptr(o), ptrs, _dptr(lam), C.byref(fit),
+                                        C.byref(its), _dptr(hist), C.c_void_p(s))
+        else:
+            hist = None
+            rc = getattr(self.lib, sym)(self.h, rank, ldm, _dptr(o), ptrs, _dptr(lam), C.byref(fit),
+                                        C.byref(its), C.c_void_p(s))
         _check(rc, sym)
-        return fit.value, lam, [b[:, :rank] for b in bufs], its.value
+        return (fit.value, lam, [b[:, :rank] for b in bufs], its.value,
+                None if hist is None else hist[:its.value].copy())
 
     def sse(self, factors, lam=None, stream=None) -> float:
         """Sum over this tensor's nonzeros of (v - sum_r lam_r prod_m factors[m][i_m, r])^2

@@ -650,6 +650,166 @@ __global__ void k_fold_lambda(double * __restrict__ lambda_total, const double *
   if (j < R) lambda_total[j] *= norms[j];
 }
 
+// ---- nonnegative CPD by HALS (Cichocki & Phan 2009; Gillis & Glineur 2012), the update step of
+// splatt_b200_cpd_nonneg_device: per mode one Gauss-Seidel sweep over the columns of
+// B = A_n diag(lambda),
+//   B[:, r] <- max(eps, (M[:, r] - sum_{j != r} B[:, j] G[j, r]) / G[r, r]),
+// G the Hadamard product of the other modes' Grams.  Rows are independent given M and G, so a
+// thread sweeps one row on its own (no atomics); the division is a product with 1 / G[r, r].
+constexpr double kHalsFloor = 1e-16;   // include/splatt_b200.h: keeps every column nonzero
+
+// G = the Hadamard product of the Grams of every mode but `mode`, full R x R (one CTA)
+__global__ void k_hals_form(const double * __restrict__ ata, int nmodes, int mode, int R,
+                            double * __restrict__ G) {
+  for (int x = threadIdx.x; x < R * R; x += blockDim.x) {
+    const int i = x / R, j = x % R;
+    const int p = min(i, j), q = max(i, j);  // Grams are stored upper (row-major)
+    double v = 1.0;
+    for (int m = 0; m < nmodes; ++m)
+      if (m != mode) v *= ata[(size_t)m * R * R + q + p * R];
+    G[x] = v;
+  }
+}
+
+// One HALS sweep per row for R <= RT (16 / 32 / 64), in place on X = A_n: one thread per row,
+// the row of B in registers (A_n[i, :] lambda in fp64), G padded to RT with zeros (1 on the pad
+// diagonal) in shared memory, read as 128-bit broadcasts; the row of M1 is loaded as the sweep
+// reaches it.  Columns [0, R) are stored once, rounded to T.  As in k_solve_rows_reg, fp32 rows
+// move as float4 and columns [R, RT) enter as 0 by selection: pad columns are loaded but never
+// feed a result or get written.
+template <int RT, class T>
+__global__ void __launch_bounds__(128)
+k_hals_rows_reg(const T * __restrict__ M1, T * __restrict__ X, unsigned long long I, int R, int ld,
+                const double * __restrict__ G, const double * __restrict__ lambda) {
+  extern __shared__ __align__(16) double sm[];
+  double * Gs  = sm;                    // RT*RT
+  double * inv = sm + RT * RT;          // 1 / G[r, r]
+  double * lam = sm + RT * RT + RT;     // lambda, 0 on the pad
+  for (int x = threadIdx.x; x < RT * RT; x += blockDim.x) {
+    const int i = x / RT, j = x % RT;
+    Gs[x] = (i < R && j < R) ? G[j + i * R] : (i == j ? 1.0 : 0.0);
+  }
+  for (int x = threadIdx.x; x < RT; x += blockDim.x) {
+    inv[x] = x < R ? 1.0 / G[x + x * R] : 1.0;
+    lam[x] = x < R ? lambda[x] : 0.0;
+  }
+  __syncthreads();
+  const unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= I) return;
+  double b[RT];
+  T * row = X + i * ld;
+  const T * m = M1 + i * ld;
+  if constexpr (sizeof(T) == 8) {
+#pragma unroll
+    for (int r = 0; r < RT; r += 2) {
+      if (r + 1 < R) {
+        const double2 v = *reinterpret_cast<const double2 *>(row + r);
+        b[r] = v.x * lam[r]; b[r + 1] = v.y * lam[r + 1];
+      } else {
+        b[r] = (r < R) ? row[r] * lam[r] : 0.0; b[r + 1] = 0.0;
+      }
+    }
+  } else {
+#pragma unroll
+    for (int r = 0; r < RT; r += 4) {
+      if (r < R) {
+        const float4 v = *reinterpret_cast<const float4 *>(row + r);
+        b[r]     = (double)v.x * lam[r];
+        b[r + 1] = (r + 1 < R) ? (double)v.y * lam[r + 1] : 0.0;
+        b[r + 2] = (r + 2 < R) ? (double)v.z * lam[r + 2] : 0.0;
+        b[r + 3] = (r + 3 < R) ? (double)v.w * lam[r + 3] : 0.0;
+      } else {
+        b[r] = b[r + 1] = b[r + 2] = b[r + 3] = 0.0;
+      }
+    }
+  }
+  double2 m2 = make_double2(0.0, 0.0);
+  float4  m4 = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+  for (int r = 0; r < RT; ++r) {
+    if (r < R) {
+      double mr;
+      if constexpr (sizeof(T) == 8) {
+        if ((r & 1) == 0) {
+          if (r + 1 < R) m2 = *reinterpret_cast<const double2 *>(m + r);
+          else m2.x = m[r];
+        }
+        mr = (r & 1) ? m2.y : m2.x;
+      } else {
+        if ((r & 3) == 0) m4 = *reinterpret_cast<const float4 *>(m + r);
+        mr = (r & 3) == 0 ? m4.x : (r & 3) == 1 ? m4.y : (r & 3) == 2 ? m4.z : m4.w;
+      }
+      // mr - sum_{j != r} B[j] G[r, j], four independent partial sums
+      double s0 = mr, s1 = 0.0, s2 = 0.0, s3 = 0.0;
+#pragma unroll
+      for (int k = 0; k < RT; k += 2) {
+        const double2 g = *reinterpret_cast<const double2 *>(&Gs[r * RT + k]);
+        if (k != r)     { if ((k & 2) == 0) s0 = fma(-g.x, b[k], s0); else s2 = fma(-g.x, b[k], s2); }
+        if (k + 1 != r) { if ((k & 2) == 0) s1 = fma(-g.y, b[k + 1], s1); else s3 = fma(-g.y, b[k + 1], s3); }
+      }
+      b[r] = fmax(kHalsFloor, ((s0 + s1) + (s2 + s3)) * inv[r]);
+    }
+  }
+  if constexpr (sizeof(T) == 8) {
+#pragma unroll
+    for (int r = 0; r < RT; r += 2) {
+      if (r + 1 < R) *reinterpret_cast<double2 *>(row + r) = make_double2(b[r], b[r + 1]);
+      else if (r < R) row[r] = b[r];
+    }
+  } else {
+#pragma unroll
+    for (int r = 0; r < RT; r += 4) {
+      if (r + 3 < R) {
+        *reinterpret_cast<float4 *>(row + r) = make_float4((float)b[r], (float)b[r + 1],
+                                                           (float)b[r + 2], (float)b[r + 3]);
+      } else {
+#pragma unroll
+        for (int c = 0; c < 3; ++c) if (r + c < R) row[r + c] = (float)b[r + c];
+      }
+    }
+  }
+}
+
+// The same sweep for any R (64 < R <= 128, or SPLATT_B200_TAIL_GENERIC=1): G in shared memory,
+// the rows of B in shared memory laid out [r][thread] (as in k_solve_rows), in place on X = A_n.
+template <class T>
+__global__ void k_hals_rows(const T * __restrict__ M1, T * __restrict__ X, unsigned long long I,
+                            int R, int ld, const double * __restrict__ G,
+                            const double * __restrict__ lambda) {
+  extern __shared__ double sm[];
+  double * Gs = sm;                         // R*R
+  double * bs = sm + R * R;                 // R * blockDim.x
+  for (int x = threadIdx.x; x < R * R; x += blockDim.x) Gs[x] = G[x];
+  __syncthreads();
+  const unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= I) return;
+  const int NT = blockDim.x, t = threadIdx.x;
+  T * row = X + i * ld;
+  const T * m = M1 + i * ld;
+  for (int r = 0; r < R; ++r) bs[r * NT + t] = static_cast<double>(row[r]) * lambda[r];
+  for (int r = 0; r < R; ++r) {
+    double s = static_cast<double>(m[r]);
+    for (int j = 0; j < r; ++j) s = fma(-Gs[j + r * R], bs[j * NT + t], s);
+    for (int j = r + 1; j < R; ++j) s = fma(-Gs[j + r * R], bs[j * NT + t], s);
+    s = fmax(kHalsFloor, s * (1.0 / Gs[r + r * R]));
+    bs[r * NT + t] = s;
+    row[r] = static_cast<T>(s);
+  }
+}
+
+// *bad = 1 if an entry (i, c), c < R, of A is negative or not finite
+template <class T>
+__global__ void k_nonneg_check(const T * __restrict__ A, unsigned long long I, int R, int ld,
+                               int * __restrict__ bad) {
+  bool b = false;
+  for (unsigned long long x = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; x < I * R;
+       x += (unsigned long long)gridDim.x * blockDim.x) {
+    const double a = static_cast<double>(A[(x / R) * ld + x % R]);
+    b |= !(a >= 0.0 && a <= 1.7976931348623157e308);
+  }
+  if (__any_sync(0xffffffffu, b) && (threadIdx.x & 31) == 0) atomicExch(bad, 1);
+}
+
 // ---- pieces of the ROW-PARTITIONED tail (multi-GPU engine, multi.cu): every device works on
 // its own row slice and publishes partial column norms / partial Grams into per-device slots
 // of the group's multicast region; all devices then combine the slots in device order, so
@@ -700,10 +860,15 @@ void with_rt(int rt, F && f) {
   else f(std::integral_constant<int, 64>());
 }
 
+// The update of a mode's factor from its MTTKRP: the ALS row solve, or the HALS sweep of the
+// nonnegative CPD.
+enum class Update { als, hals };
+
 struct DevTail {
   int N = 0, R = 0, ld = 0;
   double * ata = nullptr;     // N x R x R
   double * chol = nullptr;    // R x R
+  double * hals_g = nullptr;  // R x R: G of the HALS sweep
   double * pinv = nullptr;    // R x R
   double * lam_acc = nullptr; // R
   double * lambda = nullptr;  // R
@@ -722,6 +887,8 @@ struct DevTail {
   bool set_smem_attrs() {
     bool ok = cudaFuncSetAttribute(k_solve_rows<T>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                    (R * R + R * solve_threads) * 8) == cudaSuccess &&
+              cudaFuncSetAttribute(k_hals_rows<T>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                   (R * R + R * solve_threads) * 8) == cudaSuccess &&
               cudaFuncSetAttribute(k_gram<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, 32 * R * 8) == cudaSuccess;
     if (ok && rt) {
       const int sb = (2 * rt * rt + rt) * 8, gb = 64 * rt * 8;
@@ -739,6 +906,7 @@ struct DevTail {
     N = N_; R = R_; ld = ld_; s = st;
     bool ok = cudaMalloc(&ata, sizeof(double) * N * R * R) == cudaSuccess &&
               cudaMalloc(&chol, sizeof(double) * R * R) == cudaSuccess &&
+              cudaMalloc(&hals_g, sizeof(double) * R * R) == cudaSuccess &&
               cudaMalloc(&pinv, sizeof(double) * R * R) == cudaSuccess &&
               cudaMalloc(&lam_acc, sizeof(double) * R) == cudaSuccess &&
               cudaMalloc(&lambda, sizeof(double) * R) == cudaSuccess &&
@@ -774,7 +942,7 @@ struct DevTail {
     }
   }
   void release() {
-    cudaFree(ata); cudaFree(chol); cudaFree(pinv); cudaFree(lam_acc); cudaFree(lambda);
+    cudaFree(ata); cudaFree(chol); cudaFree(hals_g); cudaFree(pinv); cudaFree(lam_acc); cudaFree(lambda);
     cudaFree(inner); cudaFree(info); cudaFree(jac_v); cudaFree(gpart);
     if (h_back) cudaFreeHost(h_back);
   }
@@ -806,8 +974,10 @@ struct DevTail {
   }
   // one mode step after the MTTKRP: d_out (M1) -> d_mat (new factor), lambda, Gram
   template <class T>
-  void mode_step(const T * d_out, T * d_mat, uint64_t I, int m, bool two_norm) {
-    solve(d_out, d_mat, I, m);
+  void mode_step(const T * d_out, T * d_mat, uint64_t I, int m, bool two_norm,
+                 Update u = Update::als) {
+    if (u == Update::hals) hals(d_out, d_mat, I, m);
+    else solve(d_out, d_mat, I, m);
     cudaMemsetAsync(lam_acc, 0, sizeof(double) * R, s);
     dim3 g((unsigned)std::min<uint64_t>((I + 7) / 8, 1184), (R + 31) / 32);
     k_colnorm<T><<<g, 256, 0, s>>>(d_mat, I, R, ld, two_norm ? 1 : 0, lam_acc);
@@ -842,6 +1012,71 @@ struct DevTail {
     }
     check("k_solve_rows");
     spb200_count_launches(1);
+  }
+  // G of mode m, then the HALS sweep of `I` rows: d_mat (A_m) <- B, lambda read as it stands
+  template <class T>
+  void hals(const T * d_out, T * d_mat, uint64_t I, int m) {
+    k_hals_form<<<1, 256, 0, s>>>(ata, N, m, R, hals_g);
+    check("k_hals_form");
+    spb200_count_launches(1);
+    if (I == 0) return;
+    if (rt) {
+      const size_t sm = (size_t)(rt * rt + 2 * rt) * 8;
+      const unsigned nb = (unsigned)((I + 127) / 128);
+      with_rt(rt, [&](auto c) {
+        k_hals_rows_reg<decltype(c)::value, T><<<nb, 128, sm, s>>>(d_out, d_mat, I, R, ld, hals_g, lambda);
+      });
+    } else {
+      const int NT = solve_threads;
+      k_hals_rows<T><<<(unsigned)((I + NT - 1) / NT), NT, (R * R + R * NT) * 8, s>>>(
+          d_out, d_mat, I, R, ld, hals_g, lambda);
+    }
+    check("k_hals_rows");
+    spb200_count_launches(1);
+  }
+
+  // Start of the nonnegative CPD: checks every entry of columns [0, R) of the start (finite,
+  // >= 0) and its column sums of squares (positive, finite; summed into ata, before the Grams are
+  // formed), synchronising the stream once.  When they hold, 2-normalises every factor with
+  // lambda = the product of the column norms; otherwise writes nothing and returns false (as it
+  // does when a launch failed: then `failed` is set).
+  template <class T>
+  bool nonneg_start(T * const * d_mats, const uint64_t * dims) {
+    cudaMemsetAsync(info, 0, sizeof(int), s);
+    cudaMemsetAsync(ata, 0, sizeof(double) * N * R, s);
+    for (int m = 0; m < N; ++m) {
+      const uint64_t I = dims[m];
+      if (!I) continue;
+      k_nonneg_check<T><<<(unsigned)std::min<uint64_t>((I * R + 255) / 256, 1184), 256, 0, s>>>(
+          d_mats[m], I, R, ld, info);
+      dim3 g((unsigned)std::min<uint64_t>((I + 7) / 8, 1184), (R + 31) / 32);
+      k_colnorm<T><<<g, 256, 0, s>>>(d_mats[m], I, R, ld, 1, ata + (size_t)m * R);
+      spb200_count_launches(2);
+    }
+    check("start check");
+    std::vector<double> sums((size_t)N * R);
+    int bad = 1;
+    if (cudaMemcpyAsync(sums.data(), ata, sizeof(double) * N * R, cudaMemcpyDeviceToHost, s) != cudaSuccess ||
+        cudaMemcpyAsync(&bad, info, sizeof(int), cudaMemcpyDeviceToHost, s) != cudaSuccess ||
+        cudaStreamSynchronize(s) != cudaSuccess)
+      failed = true;
+    if (failed) return false;
+    for (double x : sums) bad |= !(x > 0.0 && x <= 1.7976931348623157e308);
+    if (bad) return false;
+    const std::vector<double> ones(R, 1.0);
+    if (cudaMemcpyAsync(lambda, ones.data(), sizeof(double) * R, cudaMemcpyHostToDevice, s) != cudaSuccess) {
+      failed = true;
+      return false;
+    }
+    for (int m = 0; m < N; ++m) {
+      const uint64_t I = dims[m];
+      k_finish_lambda<<<(R + 127) / 128, 128, 0, s>>>(ata + (size_t)m * R, R, 1, lam_acc);
+      k_scale_cols<T><<<(unsigned)((I * R + 255) / 256), 256, 0, s>>>(d_mats[m], I, R, ld, lam_acc);
+      k_fold_lambda<<<(R + 127) / 128, 128, 0, s>>>(lambda, lam_acc, R);
+      spb200_count_launches(3);
+    }
+    check("start normalisation");
+    return !failed;
   }
 
   // post-processing on the device (src/cpd.c:391-411): 2-normalise every factor, folding the
@@ -936,11 +1171,13 @@ int mttkrp_t(const splatt_b200_tensor * t, int m, int R, int ldm, float * const 
 // product, solver info) for the fit -- the loop's only host synchronisation.  d_mats hold the
 // start on entry (their Grams are formed here) and the factors of the last iteration on return,
 // not post-processed.  d_out: M1 scratch of max(dims) x ldm.  lambda: R host doubles, the last
-// iteration's.  false when a launch failed.
+// iteration's.  upd: the update step (Update::hals 2-normalises in every iteration and has no
+// solver info).  history: NULL or one fit per iteration run.  false when a launch failed.
 template <class T>
 bool run_device_als(const splatt_b200_tensor * t, T * const * d_mats, T * d_out, int ldm,
                     DevTail & tail, double ttnormsq, const double * options, double * lambda,
-                    double * fit_out, uint64_t * iterations_out) {
+                    double * fit_out, uint64_t * iterations_out, Update upd = Update::als,
+                    double * history = nullptr) {
   const int N = tail.N, R = tail.R;
   const uint64_t * dims = t->dims;
   AlsIterations iters(options);
@@ -952,14 +1189,16 @@ bool run_device_als(const splatt_b200_tensor * t, T * const * d_mats, T * d_out,
     iters.start();
     for (int m = 0; m < N && ok; ++m) {
       if (mttkrp_t(t, m, R, ldm, d_mats, d_out, tail.s) != SPLATT_SUCCESS) { ok = false; break; }
-      tail.mode_step(d_out, d_mats[m], dims[m], m, it == 0);
+      tail.mode_step(d_out, d_mats[m], dims[m], m, it == 0 || upd == Update::hals, upd);
     }
     if (!ok) break;
     int info_last = 0;
-    fit = tail.fit(d_mats[N - 1], d_out, dims[N - 1], ttnormsq, lambda, &info_last);
+    fit = tail.fit(d_mats[N - 1], d_out, dims[N - 1], ttnormsq, lambda,
+                   upd == Update::als ? &info_last : nullptr);
     if (tail.failed) { ok = false; break; }
     if (info_last)
       fprintf(stderr, "SPLATT: Gram matrix is not SPD. Used pseudo-inverse.\n");
+    if (history) history[it] = fit;
     its = it + 1;
     if (iters.done(it, fit)) break;
   }
@@ -968,11 +1207,12 @@ bool run_device_als(const splatt_b200_tensor * t, T * const * d_mats, T * d_out,
   return ok;
 }
 
-// splatt_b200_cpd_als_device / _f32: CPD-ALS of a device tensor from device factors.
+// splatt_b200_cpd_als_device / _f32 (Update::als) and splatt_b200_cpd_nonneg_device / _f32
+// (Update::hals): CPD of a device tensor from device factors.
 template <class T>
-int cpd_als_device(const char * name, const splatt_b200_tensor * t, int R, int ldm,
-                   const double * options, T * const * d_factors, double * lambda_out,
-                   double * fit_out, int * iterations_out, void * stream) {
+int cpd_device(const char * name, Update upd, const splatt_b200_tensor * t, int R, int ldm,
+               const double * options, T * const * d_factors, double * lambda_out,
+               double * fit_out, int * iterations_out, double * history, void * stream) {
   constexpr int align = sizeof(T) == 4 ? 4 : 2;     // row alignment of the MTTKRP
   bool bad = !t || !options || !d_factors || R < 1 || R > 128 || ldm % align != 0 ||
              ldm < (R + align - 1) / align * align;
@@ -1012,12 +1252,22 @@ int cpd_als_device(const char * name, const splatt_b200_tensor * t, int R, int l
          cudaStreamSynchronize(s) == cudaSuccess && !tail.failed;
     ttnormsq = tail.h_back[0];
   }
+  if (ok && upd == Update::hals && !tail.nonneg_start(d_factors, t->dims)) {
+    if (!tail.failed)
+      fprintf(stderr, "SPLATT: %s: a start entry is negative or not finite, or a start column is "
+                      "zero\n", name);
+    ok = false;
+  }
   ok = ok && run_device_als<T>(t, d_factors, d_out, ldm, tail, ttnormsq, options, lambda.data(),
-                               &fit, &its);
-  if (ok) {
+                               &fit, &its, upd, history);
+  if (ok && upd == Update::als) {
     ok = cudaMemcpyAsync(d_lambda, lambda.data(), sizeof(double) * R, cudaMemcpyHostToDevice, s) == cudaSuccess;
     tail.postprocess(d_factors, t->dims, d_lambda);
     ok = ok && cudaMemcpyAsync(tail.h_back, d_lambda, sizeof(double) * R, cudaMemcpyDeviceToHost, s) == cudaSuccess &&
+         cudaStreamSynchronize(s) == cudaSuccess && !tail.failed;
+  } else if (ok) {
+    // HALS leaves 2-normalised factors: lambda as the loop (or, after 0 iterations, the start) left it
+    ok = cudaMemcpyAsync(tail.h_back, tail.lambda, sizeof(double) * R, cudaMemcpyDeviceToHost, s) == cudaSuccess &&
          cudaStreamSynchronize(s) == cudaSuccess && !tail.failed;
   }
   if (ok) {
@@ -1273,16 +1523,32 @@ int splatt_b200_cpd_als_device(splatt_b200_tensor const * t, int ncolumns, int l
                                double const * options, double * const * d_factors,
                                double * lambda_out, double * fit_out, int * iterations_out,
                                void * stream) {
-  return cpd_als_device("splatt_b200_cpd_als_device", t, ncolumns, ldm, options, d_factors,
-                        lambda_out, fit_out, iterations_out, stream);
+  return cpd_device("splatt_b200_cpd_als_device", Update::als, t, ncolumns, ldm, options,
+                    d_factors, lambda_out, fit_out, iterations_out, nullptr, stream);
 }
 
 int splatt_b200_cpd_als_device_f32(splatt_b200_tensor const * t, int ncolumns, int ldm,
                                    double const * options, float * const * d_factors,
                                    double * lambda_out, double * fit_out, int * iterations_out,
                                    void * stream) {
-  return cpd_als_device("splatt_b200_cpd_als_device_f32", t, ncolumns, ldm, options, d_factors,
-                        lambda_out, fit_out, iterations_out, stream);
+  return cpd_device("splatt_b200_cpd_als_device_f32", Update::als, t, ncolumns, ldm, options,
+                    d_factors, lambda_out, fit_out, iterations_out, nullptr, stream);
+}
+
+int splatt_b200_cpd_nonneg_device(splatt_b200_tensor const * t, int ncolumns, int ldm,
+                                  double const * options, double * const * d_factors,
+                                  double * lambda_out, double * fit_out, int * iterations_out,
+                                  double * history, void * stream) {
+  return cpd_device("splatt_b200_cpd_nonneg_device", Update::hals, t, ncolumns, ldm, options,
+                    d_factors, lambda_out, fit_out, iterations_out, history, stream);
+}
+
+int splatt_b200_cpd_nonneg_device_f32(splatt_b200_tensor const * t, int ncolumns, int ldm,
+                                      double const * options, float * const * d_factors,
+                                      double * lambda_out, double * fit_out, int * iterations_out,
+                                      double * history, void * stream) {
+  return cpd_device("splatt_b200_cpd_nonneg_device_f32", Update::hals, t, ncolumns, ldm, options,
+                    d_factors, lambda_out, fit_out, iterations_out, history, stream);
 }
 
 }  // extern "C"
