@@ -199,6 +199,19 @@ def cpd_als(csf_ptr, nfactors: int, opts: np.ndarray, seed: Optional[int] = None
     return fit, lam, facs
 
 
+def _launch_args(bufs, stream, ptr_t=A.val_p):
+    """(stream handle, ctypes pointer array) for an entry point that reads the device buffers
+    `bufs`, filled on the current stream: an explicit `stream` first waits for them."""
+    import torch
+    cur = torch.cuda.current_stream(bufs[0].device)
+    if stream is None:
+        s = cur.cuda_stream
+    else:
+        cur.synchronize()    # the buffers were filled there
+        s = stream
+    return s, (ptr_t * len(bufs))(*[C.cast(C.c_void_p(b.data_ptr()), ptr_t) for b in bufs])
+
+
 class Tensor:
     """Device-resident sparse tensor (splatt_b200_tensor): per-mode fiber streams in HBM."""
 
@@ -364,6 +377,40 @@ class Tensor:
         iterations, history (numpy float64[iterations]: the fit of every iteration))."""
         return self._cpd_device(True, rank, factors, dtype, niters, tol, seed, verbosity, stream)
 
+    def _check_factors(self, factors, cols, dtype, what):
+        """Raise ValueError unless factors (None: no start given) holds one tensor of shape
+        (dims[m], cols[m]) per mode on the current device, each of `dtype` (`what`: the entry
+        point named in the error; None: the caller checked the dtypes)."""
+        import torch
+        if factors is None:
+            return
+        dev = torch.device("cuda", torch.cuda.current_device())
+        if len(factors) != self.nmodes:
+            raise ValueError(f"{len(factors)} factor matrices for a {self.nmodes}-mode tensor")
+        for m, f in enumerate(factors):
+            if what is not None and f.dtype != dtype:
+                raise ValueError(f"factor matrix {m} is {f.dtype}; {what} is float64 only")
+            if f.device != dev or tuple(f.shape) != (self.dims[m], cols[m]):
+                raise ValueError(f"factor matrix {m} must be a tensor of shape "
+                                 f"({self.dims[m]}, {cols[m]}) on the current device {dev}")
+
+    def _start_factors(self, factors, cols, ldm, dtype, seed=0, draw=None):
+        """One zero-padded (dims[m], ldm) `dtype` buffer per mode on the current device, its
+        first cols[m] columns copied from factors[m] (checked by _check_factors) or, when factors
+        is None, drawn by draw(view, generator) mode by mode from a torch.Generator seeded with
+        `seed`."""
+        import torch
+        dev = torch.device("cuda", torch.cuda.current_device())
+        bufs = [torch.zeros((d, ldm), dtype=dtype, device=dev) for d in self.dims]
+        if factors is None:
+            g = torch.Generator(device=dev).manual_seed(seed)
+            for b, r in zip(bufs, cols):
+                draw(b[:, :r], g)
+        else:
+            for b, f, r in zip(bufs, factors, cols):
+                b[:, :r].copy_(f)
+        return bufs
+
     def _cpd_device(self, nonneg, rank, factors, dtype, niters, tol, seed, verbosity, stream):
         """cpd_als (nonneg False) or cpd_nonneg: (fit, lambda, factors, iterations, history)."""
         import torch
@@ -374,41 +421,23 @@ class Tensor:
             for m, f in enumerate(factors):
                 if f.dtype != dt:
                     raise ValueError(f"factor matrix {m} is {f.dtype} but factor matrix 0 is {dt}")
-            if len(factors) != self.nmodes:
-                raise ValueError(f"{len(factors)} factor matrices for a {self.nmodes}-mode tensor")
-        dev = torch.device("cuda", torch.cuda.current_device())
-        if factors is not None:
-            for m, f in enumerate(factors):
-                if f.device != dev or tuple(f.shape) != (self.dims[m], rank):
-                    raise ValueError(f"factor matrix {m} must be a tensor of shape "
-                                     f"({self.dims[m]}, {rank}) on the current device {dev}")
         else:
             dt = torch.float64 if dtype is None else dtype
+        self._check_factors(factors, [rank] * self.nmodes, dt, None)
         if dt == torch.float64:
             ptr_t, sym, ldm = A.val_p, "splatt_b200_cpd_als_device", rank + (rank & 1)
         elif dt == torch.float32:
             ptr_t, sym, ldm = A.f32_p, "splatt_b200_cpd_als_device_f32", (rank + 3) & ~3
         else:
             raise ValueError(f"CPD factors must be float64 or float32, not {dt}")
-        bufs = [torch.zeros((d, ldm), dtype=dt, device=dev) for d in self.dims]
-        if factors is None:
-            g = torch.Generator(device=dev).manual_seed(seed)
-            lo, hi = (0.0, 1.0) if nonneg else (-3.0, 3.0)
-            for b in bufs:
-                b[:, :rank].uniform_(lo, hi, generator=g)
-        else:
-            for b, f in zip(bufs, factors):
-                b[:, :rank].copy_(f)
+        lo, hi = (0.0, 1.0) if nonneg else (-3.0, 3.0)
+        bufs = self._start_factors(factors, [rank] * self.nmodes, ldm, dt, seed,
+                                   lambda v, g: v.uniform_(lo, hi, generator=g))
         o = default_opts()
         o[A.OPTION_NITER] = niters
         o[A.OPTION_TOLERANCE] = tol
         o[A.OPTION_VERBOSITY] = verbosity
-        if stream is None:
-            s = torch.cuda.current_stream(dev).cuda_stream
-        else:
-            torch.cuda.current_stream(dev).synchronize()    # the buffers were filled there
-            s = stream
-        ptrs = (ptr_t * self.nmodes)(*[C.cast(C.c_void_p(b.data_ptr()), ptr_t) for b in bufs])
+        s, ptrs = _launch_args(bufs, stream, ptr_t)
         lam = np.zeros(rank)
         fit = C.c_double()
         its = C.c_int()
@@ -430,29 +459,14 @@ class Tensor:
         (splatt_b200_tensor_sse; lam None = all ones).  factors: float64 CUDA tensors
         (dims[m] x rank) on the current device; rank <= 64.  Synchronises the stream once."""
         import torch
-        dev = torch.device("cuda", torch.cuda.current_device())
-        if len(factors) != self.nmodes:
-            raise ValueError(f"{len(factors)} factor matrices for a {self.nmodes}-mode tensor")
-        rank = factors[0].shape[1] if factors[0].dim() == 2 else -1
-        for m, f in enumerate(factors):
-            if f.dtype != torch.float64:
-                raise ValueError(f"factor matrix {m} is {f.dtype}; Tensor.sse is float64 only")
-            if f.device != dev or tuple(f.shape) != (self.dims[m], rank):
-                raise ValueError(f"factor matrix {m} must be a tensor of shape "
-                                 f"({self.dims[m]}, {rank}) on the current device {dev}")
+        rank = factors[0].shape[1] if len(factors) == self.nmodes and factors[0].dim() == 2 else -1
+        self._check_factors(factors, [rank] * self.nmodes, torch.float64, "Tensor.sse")
         ldm = rank + (rank & 1)
-        bufs = [torch.zeros((d, ldm), dtype=torch.float64, device=dev) for d in self.dims]
-        for b, f in zip(bufs, factors):
-            b[:, :rank].copy_(f)
+        bufs = self._start_factors(factors, [rank] * self.nmodes, ldm, torch.float64)
         lam_a = None if lam is None else np.ascontiguousarray(lam, dtype=np.float64)
         if lam_a is not None and lam_a.shape != (rank,):
             raise ValueError(f"lam must have {rank} entries")
-        if stream is None:
-            s = torch.cuda.current_stream(dev).cuda_stream
-        else:
-            torch.cuda.current_stream(dev).synchronize()    # the buffers were filled there
-            s = stream
-        ptrs = (A.val_p * self.nmodes)(*[C.cast(C.c_void_p(b.data_ptr()), A.val_p) for b in bufs])
+        s, ptrs = _launch_args(bufs, stream)
         out = C.c_double()
         rc = self.lib.splatt_b200_tensor_sse(self.h, rank, ldm, ptrs,
                                              A.val_p() if lam_a is None else _dptr(lam_a),
@@ -476,38 +490,18 @@ class Tensor:
         Returns (history: numpy float64 [iterations x 3] of (objective, training RMSE,
         validation RMSE or NaN), factors (CUDA views dims[m] x rank), iterations)."""
         import torch
-        dev = torch.device("cuda", torch.cuda.current_device())
-        if factors is not None:
-            if len(factors) != self.nmodes:
-                raise ValueError(f"{len(factors)} factor matrices for a {self.nmodes}-mode tensor")
-            for m, f in enumerate(factors):
-                if f.dtype != torch.float64:
-                    raise ValueError(f"factor matrix {m} is {f.dtype}; completion is float64 only")
-                if f.device != dev or tuple(f.shape) != (self.dims[m], rank):
-                    raise ValueError(f"factor matrix {m} must be a tensor of shape "
-                                     f"({self.dims[m]}, {rank}) on the current device {dev}")
+        self._check_factors(factors, [rank] * self.nmodes, torch.float64, "completion")
         if validate is not None and not isinstance(validate, Tensor):
             raise ValueError("validate must be a Tensor")
         ldm = rank + (rank & 1)
-        bufs = [torch.zeros((d, ldm), dtype=torch.float64, device=dev) for d in self.dims]
-        if factors is None:
-            g = torch.Generator(device=dev).manual_seed(seed)
-            for b in bufs:
-                b[:, :rank].uniform_(0.0, 1.0, generator=g)
-        else:
-            for b, f in zip(bufs, factors):
-                b[:, :rank].copy_(f)
+        bufs = self._start_factors(factors, [rank] * self.nmodes, ldm, torch.float64, seed,
+                                   lambda v, g: v.uniform_(0.0, 1.0, generator=g))
         o = default_opts()
         o[A.OPTION_NITER] = niters
         o[A.OPTION_TOLERANCE] = tol
         o[A.OPTION_VERBOSITY] = verbosity
         o[A.OPTION_REGULARIZE] = reg
-        if stream is None:
-            s = torch.cuda.current_stream(dev).cuda_stream
-        else:
-            torch.cuda.current_stream(dev).synchronize()    # the buffers were filled there
-            s = stream
-        ptrs = (A.val_p * self.nmodes)(*[C.cast(C.c_void_p(b.data_ptr()), A.val_p) for b in bufs])
+        s, ptrs = _launch_args(bufs, stream)
         hist = np.full((max(int(niters), 0), 3), np.nan)
         its = C.c_int()
         rc = self.lib.splatt_b200_tc_als_device(self.h, None if validate is None else validate.h,
@@ -536,36 +530,16 @@ class Tensor:
         float64 [iterations x 3] of (log-likelihood, largest final KKT violation, inner
         iterations summed over the modes)), iterations)."""
         import torch
-        dev = torch.device("cuda", torch.cuda.current_device())
-        if factors is not None:
-            if len(factors) != self.nmodes:
-                raise ValueError(f"{len(factors)} factor matrices for a {self.nmodes}-mode tensor")
-            for m, f in enumerate(factors):
-                if f.dtype != torch.float64:
-                    raise ValueError(f"factor matrix {m} is {f.dtype}; CP-APR is float64 only")
-                if f.device != dev or tuple(f.shape) != (self.dims[m], rank):
-                    raise ValueError(f"factor matrix {m} must be a tensor of shape "
-                                     f"({self.dims[m]}, {rank}) on the current device {dev}")
+        self._check_factors(factors, [rank] * self.nmodes, torch.float64, "CP-APR")
         ldm = rank + (rank & 1)
-        bufs = [torch.zeros((d, ldm), dtype=torch.float64, device=dev) for d in self.dims]
-        if factors is None:
-            g = torch.Generator(device=dev).manual_seed(seed)
-            for b in bufs:
-                b[:, :rank].uniform_(0.0, 1.0, generator=g)
-        else:
-            for b, f in zip(bufs, factors):
-                b[:, :rank].copy_(f)
+        bufs = self._start_factors(factors, [rank] * self.nmodes, ldm, torch.float64, seed,
+                                   lambda v, g: v.uniform_(0.0, 1.0, generator=g))
         o = default_opts()
         o[A.OPTION_NITER] = niters
         o[A.OPTION_TOLERANCE] = tol
         o[A.OPTION_VERBOSITY] = verbosity
         ao = A.AprOpts(max_inner, kappa, kappa_tol, eps)
-        if stream is None:
-            s = torch.cuda.current_stream(dev).cuda_stream
-        else:
-            torch.cuda.current_stream(dev).synchronize()    # the buffers were filled there
-            s = stream
-        ptrs = (A.val_p * self.nmodes)(*[C.cast(C.c_void_p(b.data_ptr()), A.val_p) for b in bufs])
+        s, ptrs = _launch_args(bufs, stream)
         lam = np.zeros(rank)
         hist = np.full((max(int(niters), 0), 3), np.nan)
         its = C.c_int()
@@ -631,39 +605,19 @@ class Tensor:
         history (numpy float64 [iterations x 4] of (fit, ||core||_F, orthogonal-iteration steps
         summed over the modes, largest final subspace residual)), iterations)."""
         import torch
-        dev = torch.device("cuda", torch.cuda.current_device())
         ranks = [int(r) for r in ranks]
         if len(ranks) != self.nmodes:
             raise ValueError(f"{len(ranks)} ranks for a {self.nmodes}-mode tensor")
-        if factors is not None:
-            if len(factors) != self.nmodes:
-                raise ValueError(f"{len(factors)} factor matrices for a {self.nmodes}-mode tensor")
-            for m, f in enumerate(factors):
-                if f.dtype != torch.float64:
-                    raise ValueError(f"factor matrix {m} is {f.dtype}; Tucker is float64 only")
-                if f.device != dev or tuple(f.shape) != (self.dims[m], ranks[m]):
-                    raise ValueError(f"factor matrix {m} must be a tensor of shape "
-                                     f"({self.dims[m]}, {ranks[m]}) on the current device {dev}")
+        self._check_factors(factors, ranks, torch.float64, "Tucker")
         ldm = max(ranks) + (max(ranks) & 1)
-        bufs = [torch.zeros((d, ldm), dtype=torch.float64, device=dev) for d in self.dims]
-        if factors is None:
-            g = torch.Generator(device=dev).manual_seed(seed)
-            for b, r in zip(bufs, ranks):
-                b[:, :r].normal_(0.0, 1.0, generator=g)
-        else:
-            for b, f, r in zip(bufs, factors, ranks):
-                b[:, :r].copy_(f)
+        bufs = self._start_factors(factors, ranks, ldm, torch.float64, seed,
+                                   lambda v, g: v.normal_(0.0, 1.0, generator=g))
         o = default_opts()
         o[A.OPTION_NITER] = niters
         o[A.OPTION_TOLERANCE] = tol
         o[A.OPTION_VERBOSITY] = verbosity
         to = A.TuckerOpts(max_power, svd_tol)
-        if stream is None:
-            s = torch.cuda.current_stream(dev).cuda_stream
-        else:
-            torch.cuda.current_stream(dev).synchronize()    # the buffers were filled there
-            s = stream
-        ptrs = (A.val_p * self.nmodes)(*[C.cast(C.c_void_p(b.data_ptr()), A.val_p) for b in bufs])
+        s, ptrs = _launch_args(bufs, stream)
         rk = (C.c_int * self.nmodes)(*ranks)
         core = np.zeros(int(np.prod(ranks)))
         hist = np.full((max(int(niters), 0), 4), np.nan)

@@ -214,43 +214,12 @@ __global__ void __launch_bounds__(kThreads, 3) k_apr_ll(const TcArgs a) {
 
 // ---- host side ---------------------------------------------------------------------------------
 
-unsigned elementwise_grid(uint64_t rows, int R) {
-  return (unsigned)std::max<uint64_t>(std::min<uint64_t>((rows * R + kThreads - 1) / kThreads, 1184), 1);
-}
-
 // out[c] = sum over the rows of M[i, c], c < R (part: kColsumCtas x 64 doubles of scratch)
 void launch_colsum(const double * M, uint64_t rows, int R, int ldm, double * part, double * out,
                    cudaStream_t s) {
   k_apr_colsum_part<<<kColsumCtas, kThreads, 0, s>>>(M, rows, R, ldm, part);
   k_apr_colsum_fin<<<1, 64, 0, s>>>(part, kColsumCtas, R, out);
   spb200_count_launches(2);
-}
-
-template <int N>
-void (*phi_kernel_n(bool rows))(TcArgs) {
-  return rows ? k_apr_phi<N, true> : k_apr_phi<N, false>;
-}
-void (*phi_kernel(int N, bool rows))(TcArgs) {
-  switch (N) {
-    case 2: return phi_kernel_n<2>(rows);
-    case 3: return phi_kernel_n<3>(rows);
-    case 4: return phi_kernel_n<4>(rows);
-    case 5: return phi_kernel_n<5>(rows);
-    case 6: return phi_kernel_n<6>(rows);
-    case 7: return phi_kernel_n<7>(rows);
-    default: return phi_kernel_n<8>(rows);
-  }
-}
-void (*ll_kernel(int N))(TcArgs) {
-  switch (N) {
-    case 2: return k_apr_ll<2>;
-    case 3: return k_apr_ll<3>;
-    case 4: return k_apr_ll<4>;
-    case 5: return k_apr_ll<5>;
-    case 6: return k_apr_ll<6>;
-    case 7: return k_apr_ll<7>;
-    default: return k_apr_ll<8>;
-  }
 }
 
 // Device buffers of one CP-APR run, released on every return path.
@@ -286,17 +255,11 @@ extern "C" int splatt_b200_cp_apr_device(splatt_b200_tensor const * t, int ncolu
   const double tol = options ? options[SPLATT_OPTION_TOLERANCE] : 0.0;
   const double niter = options ? options[SPLATT_OPTION_NITER] : 0.0;
   auto nonneg = [](double x) { return std::isfinite(x) && x >= 0.0; };
-  bool bad = !t || !options || !lambda_out || t->nmodes < 2 || t->nmodes > SPB200_MAXN ||
+  bool bad = !root_streams_ok(t) || !options || !lambda_out ||
              !factors_ok(t->nmodes, R, ldm, reinterpret_cast<const void * const *>(d_factors)) ||
-             t->shard_count > 1 || t->layout != SPLATT_B200_LAYOUT_ALLROOT || t->streams.empty() ||
              o.max_inner < 1 || !nonneg(o.kappa) || !nonneg(o.kappa_tol) ||
              !(std::isfinite(o.eps_div_zero) && o.eps_div_zero > 0.0) || !nonneg(tol) ||
              !(niter >= 0.0 && niter <= 2147483647.0);
-  for (int m = 0; !bad && m < t->nmodes; ++m) {
-    const ModePlan & p = t->plan[m];
-    bad = p.stream < 0 || p.stream >= (int)t->streams.size() || p.kind != SPB200_KIND_ROOT ||
-          t->streams[p.stream].perm[0] != m || !stream_fits(t->streams[p.stream]);
-  }
   if (bad) {
     fprintf(stderr, "SPLATT: splatt_b200_cp_apr_device: bad arguments\n");
     return SPLATT_ERROR_BADINPUT;
@@ -310,29 +273,23 @@ extern "C" int splatt_b200_cp_apr_device(splatt_b200_tensor const * t, int ncolu
   const int verbosity = (int)options[SPLATT_OPTION_VERBOSITY];
 
   // one Phi launch configuration per mode; the slot buffer serves the largest
-  struct ModeLaunch { void (*k)(TcArgs); int grid; bool rows; };
-  ModeLaunch ml[SPB200_MAXN];
-  const size_t smem = tc_ring_bytes();
-  size_t max_slots = 1;
+  WalkLaunch<TcArgs> ml[SPB200_MAXN];
   uint64_t max_dim = 1;
   for (int m = 0; m < N; ++m) {
-    ml[m].rows = t->streams[t->plan[m].stream].ktile_rows > 0;
-    ml[m].k = phi_kernel(N, ml[m].rows);
-    int nb = 0;
-    if (cudaFuncSetAttribute(ml[m].k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess ||
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, ml[m].k, kThreads, smem) != cudaSuccess) {
+    const bool rows = t->streams[t->plan[m].stream].ktile_rows > 0;
+    auto phi = [rows](auto n) { return rows ? k_apr_phi<n.value, true> : k_apr_phi<n.value, false>; };
+    if (!ml[m].configure(with_nmodes(N, phi), tc_ring_bytes(), rows)) {
       fprintf(stderr, "SPLATT: splatt_b200_cp_apr_device: cannot configure the Phi kernel (%s)\n",
               cudaGetErrorString(cudaGetLastError()));
       return SPLATT_ERROR_BADINPUT;
     }
-    ml[m].grid = std::max(nb, 1) * num_sms();
-    max_slots = std::max<size_t>(max_slots, 2 * (size_t)ml[m].grid * kWarps);
     max_dim = std::max<uint64_t>(max_dim, t->dims[m]);
   }
+  const unsigned long long max_slot = std::max(max_slots(ml, N), 1ull);
   AprBuffers b;
   bool ok = cudaMalloc(&b.B, max_dim * ldm * sizeof(double)) == cudaSuccess &&
-            cudaMalloc(&b.packs, max_slots * RP * sizeof(double)) == cudaSuccess &&
-            cudaMalloc(&b.slot_row, max_slots * sizeof(uint32_t)) == cudaSuccess &&
+            cudaMalloc(&b.packs, max_slot * RP * sizeof(double)) == cudaSuccess &&
+            cudaMalloc(&b.slot_row, max_slot * sizeof(uint32_t)) == cudaSuccess &&
             cudaMalloc(&b.lam, RP * sizeof(double)) == cudaSuccess &&
             cudaMalloc(&b.sums, (size_t)N * RP * sizeof(double)) == cudaSuccess &&
             cudaMalloc(&b.ll, sizeof(double)) == cudaSuccess &&
@@ -404,18 +361,15 @@ extern "C" int splatt_b200_cp_apr_device(splatt_b200_tensor const * t, int ncolu
     int inner_total = 0;
     for (int n = 0; ok && n < N; ++n) {
       const FiberStream & fs = t->streams[t->plan[n].stream];
-      const ModeLaunch & L = ml[n];
+      const WalkLaunch<TcArgs> & L = ml[n];
       const uint64_t rows = t->dims[n];
       const unsigned eg = elementwise_grid(rows, R);
-      const unsigned long long nslots = 2ull * L.grid * kWarps;
       k_apr_scale<<<eg, kThreads, 0, s>>>(d_factors[n], b.phi[n], b.lam, b.B, rows, R, ldm, o.kappa,
                                           o.kappa_tol, it > 0);
       spb200_count_launches(1);
-      TcArgs a = {};
-      fill_stream_args(fs, a);
+      TcArgs a = walk_args(fs, d_factors, ldm, R);
       a.mats[0] = b.B;
-      for (int l = 1; l < N; ++l) a.mats[l] = d_factors[fs.perm[l]];
-      a.ldm = ldm; a.R = R; a.eps = o.eps_div_zero; a.out = b.phi[n];
+      a.eps = o.eps_div_zero; a.out = b.phi[n];
       a.packs = b.packs; a.slot_row = b.slot_row;
       double kkt = 0.0;
       int l = 0;
@@ -423,13 +377,10 @@ extern "C" int splatt_b200_cp_apr_device(splatt_b200_tensor const * t, int ncolu
         ok = cudaMemsetAsync(b.phi[n], 0, rows * ldm * sizeof(double), s) == cudaSuccess &&
              cudaMemsetAsync(b.kkt, 0, sizeof(unsigned long long), s) == cudaSuccess;
         if (ok && fs.nrec) {
-          if (!L.rows) ok = cudaMemsetAsync(b.slot_row, 0xff, nslots * sizeof(uint32_t), s) == cudaSuccess;
-          L.k<<<L.grid, kThreads, smem, s>>>(a);
-          spb200_count_launches(1);
-          if (!L.rows) {
-            const unsigned cg = (unsigned)std::min<unsigned long long>((nslots + kWarps - 1) / kWarps,
-                                                                       (unsigned long long)num_sms() * 8);
-            k_apr_combine<<<cg, kThreads, 0, s>>>(b.packs, b.slot_row, nslots, R, ldm, b.phi[n]);
+          ok = L.launch(a, b.slot_row, s) == cudaSuccess;
+          if (ok && !L.rows) {
+            k_apr_combine<<<combine_grid(L.nslots), kThreads, 0, s>>>(b.packs, b.slot_row, L.nslots, R, ldm,
+                                                                      b.phi[n]);
             spb200_count_launches(1);
           }
         }
@@ -458,11 +409,9 @@ extern "C" int splatt_b200_cp_apr_device(splatt_b200_tensor const * t, int ncolu
     double ll = 0.0;
     ok = cudaMemsetAsync(b.ll, 0, sizeof(double), s) == cudaSuccess;
     if (ok && fs0.nrec) {
-      TcArgs a = {};
-      fill_stream_args(fs0, a);
-      for (int l = 0; l < N; ++l) a.mats[l] = d_factors[fs0.perm[l]];
-      a.ldm = ldm; a.R = R; a.lambda = b.lam; a.sse = b.ll; a.eps = o.eps_div_zero;
-      ok = launch_model_sum(ll_kernel(N), a, s) == cudaSuccess;
+      TcArgs a = walk_args(fs0, d_factors, ldm, R);
+      a.lambda = b.lam; a.sse = b.ll; a.eps = o.eps_div_zero;
+      ok = launch_model_sum(with_nmodes(N, [](auto n) { return k_apr_ll<n.value>; }), a, s) == cudaSuccess;
     }
     ok = ok && cudaMemcpyAsync(&ll, b.ll, sizeof(double), cudaMemcpyDeviceToHost, s) == cudaSuccess &&
          cudaMemcpyAsync(lam.data(), b.lam, RP * sizeof(double), cudaMemcpyDeviceToHost, s) == cudaSuccess &&

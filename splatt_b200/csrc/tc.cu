@@ -253,35 +253,12 @@ __global__ void __launch_bounds__(kThreads) k_tc_sumsq(const double * __restrict
 
 int rank_tier(int R) { return R <= 16 ? 16 : (R <= 32 ? 32 : 64); }
 
-// Kernel pointer and grid (resident CTAs) of the row update for (N, tier, rows mode).
-template <int N, int RT, bool ROWS>
-cudaError_t update_kernel_of(void (**k)(TcArgs), size_t * smem, int * grid) {
-  *k    = k_tc_update<N, RT, ROWS>;
-  *smem = tc_update_smem(RT);
-  cudaError_t e = cudaFuncSetAttribute(*k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)*smem);
-  if (e != cudaSuccess) return e;
-  int nb = 0;
-  e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, *k, kThreads, *smem);
-  *grid = std::max(nb, 1) * num_sms();
-  return e;
-}
+// The row-update kernel of (N, tier, rows mode).
 template <int N>
-cudaError_t update_kernel_n(int RT, bool rows, void (**k)(TcArgs), size_t * smem, int * grid) {
-  if (RT == 16) return rows ? update_kernel_of<N, 16, true>(k, smem, grid) : update_kernel_of<N, 16, false>(k, smem, grid);
-  if (RT == 32) return rows ? update_kernel_of<N, 32, true>(k, smem, grid) : update_kernel_of<N, 32, false>(k, smem, grid);
-  return rows ? update_kernel_of<N, 64, true>(k, smem, grid) : update_kernel_of<N, 64, false>(k, smem, grid);
-}
-cudaError_t update_kernel(int N, int R, bool rows, void (**k)(TcArgs), size_t * smem, int * grid) {
-  const int RT = rank_tier(R);
-  switch (N) {
-    case 2: return update_kernel_n<2>(RT, rows, k, smem, grid);
-    case 3: return update_kernel_n<3>(RT, rows, k, smem, grid);
-    case 4: return update_kernel_n<4>(RT, rows, k, smem, grid);
-    case 5: return update_kernel_n<5>(RT, rows, k, smem, grid);
-    case 6: return update_kernel_n<6>(RT, rows, k, smem, grid);
-    case 7: return update_kernel_n<7>(RT, rows, k, smem, grid);
-    default: return update_kernel_n<8>(RT, rows, k, smem, grid);
-  }
+void (*update_kernel(int RT, bool rows))(TcArgs) {
+  if (RT == 16) return rows ? k_tc_update<N, 16, true> : k_tc_update<N, 16, false>;
+  if (RT == 32) return rows ? k_tc_update<N, 32, true> : k_tc_update<N, 32, false>;
+  return rows ? k_tc_update<N, 64, true> : k_tc_update<N, 64, false>;
 }
 
 cudaError_t launch_solve(const double * packs, const uint32_t * slot_row, unsigned long long nitems,
@@ -293,9 +270,7 @@ cudaError_t launch_solve(const double * packs, const uint32_t * slot_row, unsign
       RT == 16 ? k_tc_solve<16> : (RT == 32 ? k_tc_solve<32> : k_tc_solve<64>);
   cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return e;
-  const unsigned long long want = (nitems + kWarps - 1) / kWarps;
-  const unsigned grid = (unsigned)std::min<unsigned long long>(want, (unsigned long long)num_sms() * 8);
-  k<<<grid, kThreads, smem, s>>>(packs, slot_row, nitems, R, ldm, reg, out);
+  k<<<combine_grid(nitems), kThreads, smem, s>>>(packs, slot_row, nitems, R, ldm, reg, out);
   spb200_count_launches(1);
   return cudaGetLastError();
 }
@@ -304,21 +279,9 @@ cudaError_t launch_solve(const double * packs, const uint32_t * slot_row, unsign
 cudaError_t launch_sse(const FiberStream & fs, int R, int ldm, const double * const * d_mats_by_mode,
                        const double * d_lambda, double * d_sse, cudaStream_t s) {
   if (fs.nrec == 0) return cudaSuccess;
-  TcArgs a = {};
-  fill_stream_args(fs, a);
-  for (int l = 0; l < fs.nmodes; ++l) a.mats[l] = d_mats_by_mode[fs.perm[l]];
-  a.ldm = ldm; a.R = R; a.lambda = d_lambda; a.sse = d_sse;
-  void (*k)(TcArgs) = nullptr;
-  switch (fs.nmodes) {
-    case 2: k = k_tc_sse<2>; break;
-    case 3: k = k_tc_sse<3>; break;
-    case 4: k = k_tc_sse<4>; break;
-    case 5: k = k_tc_sse<5>; break;
-    case 6: k = k_tc_sse<6>; break;
-    case 7: k = k_tc_sse<7>; break;
-    default: k = k_tc_sse<8>; break;
-  }
-  return launch_model_sum(k, a, s);
+  TcArgs a = walk_args(fs, d_mats_by_mode, ldm, R);
+  a.lambda = d_lambda; a.sse = d_sse;
+  return launch_model_sum(with_nmodes(fs.nmodes, [](auto n) { return k_tc_sse<n.value>; }), a, s);
 }
 
 // Device buffers of one completion run, released on every return path.
@@ -373,15 +336,9 @@ extern "C" int splatt_b200_tc_als_device(splatt_b200_tensor const * train,
                                          double * history, int * iterations_out, void * stream) {
   const int R = ncolumns;
   const double reg = options ? options[SPLATT_OPTION_REGULARIZE] : 0.0;
-  bool bad = !train || !options || train->nmodes < 2 || train->nmodes > SPB200_MAXN ||
+  bool bad = !root_streams_ok(train) || !options ||
              !factors_ok(train->nmodes, R, ldm, reinterpret_cast<const void * const *>(d_factors)) ||
-             !(std::isfinite(reg) && reg > 0.0) || train->shard_count > 1 ||
-             train->layout != SPLATT_B200_LAYOUT_ALLROOT || train->streams.empty();
-  for (int m = 0; !bad && m < train->nmodes; ++m) {
-    const ModePlan & p = train->plan[m];
-    bad = p.stream < 0 || p.stream >= (int)train->streams.size() || p.kind != SPB200_KIND_ROOT ||
-          train->streams[p.stream].perm[0] != m || !stream_fits(train->streams[p.stream]);
-  }
+             !(std::isfinite(reg) && reg > 0.0);
   if (!bad && validate) {
     bad = validate->nmodes != train->nmodes || validate->shard_count > 1 ||
           validate->device != train->device || validate->streams.empty() ||
@@ -402,27 +359,26 @@ extern "C" int splatt_b200_tc_als_device(splatt_b200_tensor const * train,
   const double tol = options[SPLATT_OPTION_TOLERANCE];
   const int verbosity = (int)options[SPLATT_OPTION_VERBOSITY];
 
-  // one launch configuration per mode; the pack buffer serves the largest
-  struct ModeLaunch { void (*k)(TcArgs); size_t smem; int grid; bool rows; };
-  ModeLaunch ml[SPB200_MAXN];
-  size_t max_packs = 0, max_slots = 0;
+  // one launch configuration per mode; the pack buffer serves the largest (a leaf-tiled mode: a
+  // pack per row)
+  const int RT = rank_tier(R);
+  WalkLaunch<TcArgs> ml[SPB200_MAXN];
+  size_t max_packs = 0;
   for (int m = 0; m < N; ++m) {
-    const FiberStream & fs = train->streams[train->plan[m].stream];
-    ml[m].rows = fs.ktile_rows > 0;
-    if (update_kernel(N, R, ml[m].rows, &ml[m].k, &ml[m].smem, &ml[m].grid) != cudaSuccess) {
+    const bool rows = train->streams[train->plan[m].stream].ktile_rows > 0;
+    if (!ml[m].configure(with_nmodes(N, [&](auto n) { return update_kernel<n.value>(RT, rows); }),
+                         tc_update_smem(RT), rows)) {
       fprintf(stderr, "SPLATT: splatt_b200_tc_als_device: cannot configure the row update (%s)\n",
               cudaGetErrorString(cudaGetLastError()));
       return SPLATT_ERROR_BADINPUT;
     }
-    const size_t slots = 2 * (size_t)ml[m].grid * kWarps;
-    max_packs = std::max<size_t>(max_packs, ml[m].rows ? train->dims[m] : slots);
-    if (!ml[m].rows) max_slots = std::max(max_slots, slots);
+    max_packs = std::max<size_t>(max_packs, rows ? train->dims[m] : ml[m].nslots);
   }
   TcBuffers b;
   std::vector<double> ones(RP, 0.0);
   std::fill(ones.begin(), ones.begin() + R, 1.0);
   if (cudaMalloc(&b.packs, std::max<size_t>(max_packs, 1) * P * sizeof(double)) != cudaSuccess ||
-      cudaMalloc(&b.slot_row, std::max<size_t>(max_slots, 1) * sizeof(uint32_t)) != cudaSuccess ||
+      cudaMalloc(&b.slot_row, std::max(max_slots(ml, N), 1ull) * sizeof(uint32_t)) != cudaSuccess ||
       cudaMalloc(&b.lambda, RP * sizeof(double)) != cudaSuccess ||
       cudaMalloc(&b.sums, 3 * sizeof(double)) != cudaSuccess) {
     cudaGetLastError();
@@ -438,32 +394,26 @@ extern "C" int splatt_b200_tc_als_device(splatt_b200_tensor const * train,
     if (verbosity > SPLATT_VERBOSITY_NONE) t0 = std::chrono::steady_clock::now();
     for (int m = 0; ok && m < N; ++m) {
       const FiberStream & fs = train->streams[train->plan[m].stream];
-      const ModeLaunch & L = ml[m];
+      const WalkLaunch<TcArgs> & L = ml[m];
       ok = cudaMemset2DAsync(d_factors[m], (size_t)ldm * 8, 0, (size_t)R * 8, train->dims[m], s) == cudaSuccess;
-      const unsigned long long nslots = 2ull * L.grid * kWarps;
       if (L.rows) ok = ok && cudaMemsetAsync(b.packs, 0, train->dims[m] * P * sizeof(double), s) == cudaSuccess;
-      else ok = ok && cudaMemsetAsync(b.slot_row, 0xff, nslots * sizeof(uint32_t), s) == cudaSuccess;
       if (!ok) break;
       if (fs.nrec) {
-        TcArgs a = {};
-        fill_stream_args(fs, a);
-        for (int l = 0; l < N; ++l) a.mats[l] = d_factors[fs.perm[l]];
-        a.ldm = ldm; a.R = R; a.reg = reg; a.out = d_factors[m];
+        TcArgs a = walk_args(fs, d_factors, ldm, R);
+        a.reg = reg; a.out = d_factors[m];
         a.packs = b.packs; a.slot_row = L.rows ? nullptr : b.slot_row;
-        L.k<<<L.grid, kThreads, L.smem, s>>>(a);
-        spb200_count_launches(1);
-        ok = cudaGetLastError() == cudaSuccess;
+        ok = L.launch(a, b.slot_row, s) == cudaSuccess;
       }
       if (L.rows)
         ok = ok && launch_solve(b.packs, nullptr, train->dims[m], R, ldm, reg, d_factors[m], s) == cudaSuccess;
       else if (fs.nrec)
-        ok = ok && launch_solve(b.packs, b.slot_row, nslots, R, ldm, reg, d_factors[m], s) == cudaSuccess;
+        ok = ok && launch_solve(b.packs, b.slot_row, L.nslots, R, ldm, reg, d_factors[m], s) == cudaSuccess;
     }
     if (!ok) break;
     ok = cudaMemsetAsync(b.sums, 0, 3 * sizeof(double), s) == cudaSuccess;
     for (int m = 0; ok && m < N; ++m) {
-      const unsigned grid = (unsigned)std::min<uint64_t>((train->dims[m] * R + kThreads - 1) / kThreads, 1184);
-      k_tc_sumsq<<<std::max(grid, 1u), kThreads, 0, s>>>(d_factors[m], train->dims[m], R, ldm, b.sums + 2);
+      k_tc_sumsq<<<elementwise_grid(train->dims[m], R), kThreads, 0, s>>>(d_factors[m], train->dims[m], R, ldm,
+                                                                          b.sums + 2);
       spb200_count_launches(1);
       ok = cudaGetLastError() == cudaSuccess;
     }

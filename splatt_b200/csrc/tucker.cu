@@ -429,26 +429,12 @@ __global__ void __launch_bounds__(kThreads) k_flip_cols(double * __restrict__ M,
 
 // ---- host side ---------------------------------------------------------------------------------
 
-template <int N, int TT>
-void (*ttmc_kernel_nt(bool rows))(TtmcArgs) {
-  return rows ? k_ttmc<N, TT, true> : k_ttmc<N, TT, false>;
-}
+// The TTMc kernel of (N, register tile for C columns, rows mode).
 template <int N>
-void (*ttmc_kernel_n(int C, bool rows))(TtmcArgs) {
-  if (C <= 64) return ttmc_kernel_nt<N, 2>(rows);
-  if (C <= 256) return ttmc_kernel_nt<N, 8>(rows);
-  return ttmc_kernel_nt<N, 32>(rows);
-}
-void (*ttmc_kernel(int N, int C, bool rows))(TtmcArgs) {
-  switch (N) {
-    case 2: return ttmc_kernel_n<2>(C, rows);
-    case 3: return ttmc_kernel_n<3>(C, rows);
-    case 4: return ttmc_kernel_n<4>(C, rows);
-    case 5: return ttmc_kernel_n<5>(C, rows);
-    case 6: return ttmc_kernel_n<6>(C, rows);
-    case 7: return ttmc_kernel_n<7>(C, rows);
-    default: return ttmc_kernel_n<8>(C, rows);
-  }
+void (*ttmc_kernel(int C, bool rows))(TtmcArgs) {
+  if (C <= 64) return rows ? k_ttmc<N, 2, true> : k_ttmc<N, 2, false>;
+  if (C <= 256) return rows ? k_ttmc<N, 8, true> : k_ttmc<N, 8, false>;
+  return rows ? k_ttmc<N, 32, true> : k_ttmc<N, 32, false>;
 }
 
 int cols_but(int N, const int * ranks, int n) {
@@ -458,14 +444,9 @@ int cols_but(int N, const int * ranks, int n) {
   return C;
 }
 
-// The launch of one mode's TTMc: kernel, grid, shared memory, and its boundary-slot count.
-struct TtmcPlan {
-  void (*k)(TtmcArgs) = nullptr;
+// The launch of one mode's TTMc and its arguments.
+struct TtmcPlan : WalkLaunch<TtmcArgs> {
   TtmcArgs a = {};
-  int      grid = 0;
-  size_t   smem = 0;
-  bool     rows = false;
-  unsigned long long nslots = 0;
 };
 
 bool plan_ttmc(const splatt_b200_tensor * t, int n, const int * ranks, int ldm,
@@ -474,8 +455,7 @@ bool plan_ttmc(const splatt_b200_tensor * t, int n, const int * ranks, int ldm,
   const FiberStream & fs = t->streams[t->plan[n].stream];
   TtmcArgs & a = p.a;
   a = {};
-  fill_stream_args(fs, a.t);
-  a.t.ldm = ldm;
+  a.t = walk_args(fs, mats_by_mode, ldm, 0);
   a.t.out = out;
   int stride[SPB200_MAXN];
   for (int m = N - 1, s = 1; m >= 0; --m) {
@@ -484,7 +464,6 @@ bool plan_ttmc(const splatt_b200_tensor * t, int n, const int * ranks, int ldm,
   }
   for (int l = 0; l < N; ++l) {
     const int m = fs.perm[l];
-    a.t.mats[l] = mats_by_mode[m];
     a.rk[l] = ranks[m];
     a.cs[l] = stride[m];
   }
@@ -492,17 +471,12 @@ bool plan_ttmc(const splatt_b200_tensor * t, int n, const int * ranks, int ldm,
   a.K = (N >= 3) ? a.rk[N - 2] * a.rk[N - 1] : a.rk[1];
   a.PA = a.C / a.K;
   a.wsm = a.PA + a.K + 64 + std::max(N - 3, 0) * 32;
-  p.rows = fs.ktile_rows > 0;
-  p.k = ttmc_kernel(N, a.C, p.rows);
-  p.smem = tc_ring_bytes() + colmap_bytes(a.C) + (size_t)kWarps * a.wsm * sizeof(double);
-  int nb = 0;
-  if (cudaFuncSetAttribute(p.k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p.smem) != cudaSuccess ||
-      cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, p.k, kThreads, p.smem) != cudaSuccess || nb < 1) {
+  const bool rows = fs.ktile_rows > 0;
+  if (!p.configure(with_nmodes(N, [&](auto nm) { return ttmc_kernel<nm.value>(a.C, rows); }),
+                   tc_ring_bytes() + colmap_bytes(a.C) + (size_t)kWarps * a.wsm * sizeof(double), rows)) {
     fprintf(stderr, "SPLATT: cannot configure the TTMc kernel (%s)\n", cudaGetErrorString(cudaGetLastError()));
     return false;
   }
-  p.grid = nb * num_sms();
-  p.nslots = p.rows ? 0 : 2ull * p.grid * kWarps;
   return true;
 }
 
@@ -514,31 +488,15 @@ bool run_ttmc(const splatt_b200_tensor * t, int n, TtmcPlan & p, double * packs,
   if (!fs.nrec) return true;
   p.a.t.packs = packs;
   p.a.t.slot_row = slot_row;
-  if (!p.rows && cudaMemsetAsync(slot_row, 0xff, p.nslots * sizeof(uint32_t), s) != cudaSuccess) return false;
   // other modes may share this instantiation with less shared memory: set it for this launch
-  if (cudaFuncSetAttribute(p.k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p.smem) != cudaSuccess) return false;
-  p.k<<<p.grid, kThreads, p.smem, s>>>(p.a);
-  spb200_count_launches(1);
+  if (cudaFuncSetAttribute(p.k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p.smem) != cudaSuccess ||
+      p.launch(p.a, slot_row, s) != cudaSuccess)
+    return false;
   if (!p.rows) {
-    const unsigned cg = (unsigned)std::min<unsigned long long>((p.nslots + kWarps - 1) / kWarps,
-                                                               (unsigned long long)num_sms() * 8);
-    k_ttmc_combine<<<cg, kThreads, 0, s>>>(packs, slot_row, p.nslots, p.a.C, p.a.t.out);
+    k_ttmc_combine<<<combine_grid(p.nslots), kThreads, 0, s>>>(packs, slot_row, p.nslots, p.a.C, p.a.t.out);
     spb200_count_launches(1);
   }
   return cudaGetLastError() == cudaSuccess;
-}
-
-bool tensor_ok(const splatt_b200_tensor * t) {
-  if (!t || t->nmodes < 2 || t->nmodes > SPB200_MAXN || t->shard_count > 1 ||
-      t->layout != SPLATT_B200_LAYOUT_ALLROOT || t->streams.empty())
-    return false;
-  for (int m = 0; m < t->nmodes; ++m) {
-    const ModePlan & p = t->plan[m];
-    if (p.stream < 0 || p.stream >= (int)t->streams.size() || p.kind != SPB200_KIND_ROOT ||
-        t->streams[p.stream].perm[0] != m || !stream_fits(t->streams[p.stream]))
-      return false;
-  }
-  return true;
 }
 
 bool ranks_ok(const splatt_b200_tensor * t, const int * ranks, int ldm, bool all_modes, int mode) {
@@ -622,8 +580,7 @@ struct Dense {
     spb200_count_launches(2);
   }
   void flip(double * M, int ld, int J, uint64_t rows, const double * sgn, cudaStream_t s) {
-    k_flip_cols<<<(unsigned)std::max<uint64_t>(1, std::min<uint64_t>((rows * J + kThreads - 1) / kThreads, 1184)),
-                  kThreads, 0, s>>>(M, ld, J, rows, sgn);
+    k_flip_cols<<<elementwise_grid(rows, J), kThreads, 0, s>>>(M, ld, J, rows, sgn);
     spb200_count_launches(1);
   }
 };
@@ -649,7 +606,7 @@ using namespace spb200;
 
 extern "C" int splatt_b200_ttmc(splatt_b200_tensor const * t, int mode, int const * ranks, int ldm,
                                 double const * const * d_mats, double * d_out, void * stream) {
-  bool bad = !tensor_ok(t) || mode < 0 || mode >= t->nmodes || !d_mats || !aligned(d_out) ||
+  bool bad = !root_streams_ok(t) || mode < 0 || mode >= t->nmodes || !d_mats || !aligned(d_out) ||
              !ranks_ok(t, ranks, ldm, false, mode);
   for (int m = 0; !bad && m < t->nmodes; ++m)
     if (m != mode && !aligned(d_mats[m])) bad = true;
@@ -705,7 +662,7 @@ extern "C" int splatt_b200_tucker_hooi_device(splatt_b200_tensor const * t, int 
   const splatt_b200_tucker_opts o = topts ? *topts : splatt_b200_tucker_opts{50, 1e-10};
   const double tol = options ? options[SPLATT_OPTION_TOLERANCE] : 0.0;
   const double niter = options ? options[SPLATT_OPTION_NITER] : 0.0;
-  bool bad = !tensor_ok(t) || !options || !core_out || !d_factors || !ranks_ok(t, ranks, ldm, true, 0) ||
+  bool bad = !root_streams_ok(t) || !options || !core_out || !d_factors || !ranks_ok(t, ranks, ldm, true, 0) ||
              o.max_power < 1 || !(std::isfinite(o.svd_tol) && o.svd_tol >= 0.0) ||
              !(std::isfinite(tol) && tol >= 0.0) || !(niter >= 0.0 && niter <= 2147483647.0);
   for (int m = 0; !bad && m < t->nmodes; ++m)
@@ -726,7 +683,7 @@ extern "C" int splatt_b200_tucker_hooi_device(splatt_b200_tensor const * t, int 
   HooiBuffers b;
   Dense d;
   uint64_t max_dim = 1, max_yc = 1;
-  unsigned long long max_slots = 1;
+  unsigned long long max_packs = 1;
   int max_c = 1;
   bool ok = d.alloc();
   for (int m = 0; ok && m < N; ++m) {
@@ -750,10 +707,10 @@ extern "C" int splatt_b200_tucker_hooi_device(splatt_b200_tensor const * t, int 
   for (int m = 0; m < N; ++m) fmats[m] = b.F[m];
   for (int n = 0; n < N; ++n) {
     if (!plan_ttmc(t, n, ranks, ldm, fmats, b.Y, plan[n])) return SPLATT_ERROR_BADINPUT;
-    max_slots = std::max(max_slots, plan[n].nslots * (unsigned long long)plan[n].a.C);
+    max_packs = std::max(max_packs, plan[n].nslots * (unsigned long long)plan[n].a.C);
   }
-  if (cudaMalloc(&b.packs, max_slots * sizeof(double)) != cudaSuccess ||
-      cudaMalloc(&b.slot_row, max_slots * sizeof(uint32_t)) != cudaSuccess) {
+  if (cudaMalloc(&b.packs, max_packs * sizeof(double)) != cudaSuccess ||
+      cudaMalloc(&b.slot_row, std::max(max_slots(plan, N), 1ull) * sizeof(uint32_t)) != cudaSuccess) {
     cudaGetLastError();
     return SPLATT_ERROR_NOMEMORY;
   }

@@ -6,6 +6,7 @@
 #pragma once
 #include "mttkrp_kernels.cuh"
 #include <algorithm>
+#include <type_traits>
 
 namespace spb200 {
 namespace {
@@ -264,25 +265,104 @@ int num_sms() {
   return n;
 }
 
-void fill_stream_args(const FiberStream & fs, TcArgs & a) {
+// Calls f(std::integral_constant<int, N>{}) for the runtime mode count N in 2..SPB200_MAXN: the
+// walker kernels are instantiated per mode count.
+template <class F>
+auto with_nmodes(int N, F && f) {
+  switch (N) {
+    case 2: return f(std::integral_constant<int, 2>{});
+    case 3: return f(std::integral_constant<int, 3>{});
+    case 4: return f(std::integral_constant<int, 4>{});
+    case 5: return f(std::integral_constant<int, 5>{});
+    case 6: return f(std::integral_constant<int, 6>{});
+    case 7: return f(std::integral_constant<int, 7>{});
+    default: return f(std::integral_constant<int, 8>{});
+  }
+}
+
+// Sets kernel k's dynamic shared memory to smem bytes and returns the grid of every CTA that can
+// be resident at that size, or 0 when k cannot run with it.
+template <class Args>
+int resident_grid(void (*k)(Args), size_t smem) {
+  int nb = 0;
+  if (cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess ||
+      cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k, kThreads, smem) != cudaSuccess || nb < 1)
+    return 0;
+  return nb * num_sms();
+}
+
+// Grid of a kernel that combines boundary slots or solves rows: one warp per item, at most 8 CTAs
+// per SM.
+unsigned combine_grid(unsigned long long nitems) {
+  return (unsigned)std::min<unsigned long long>((nitems + kWarps - 1) / kWarps, (unsigned long long)num_sms() * 8);
+}
+
+// One mode's walker launch on its resident grid.  On an untiled stream (rows false) every warp
+// stores the first and the last slice of its range into its two boundary slots, and a combine
+// (or solve) kernel adds each row's slots; a leaf-tiled stream adds every piece into its row with
+// red.add and uses none.
+template <class Args>
+struct WalkLaunch {
+  void (*k)(Args) = nullptr;
+  size_t smem = 0;
+  int    grid = 0;
+  bool   rows = false;
+  unsigned long long nslots = 0;
+
+  bool configure(void (*kernel)(Args), size_t smem_bytes, bool leaf_tiled) {
+    k      = kernel;
+    smem   = smem_bytes;
+    rows   = leaf_tiled;
+    grid   = resident_grid(k, smem);
+    nslots = rows ? 0 : 2ull * grid * kWarps;
+    return grid > 0;
+  }
+  // Marks every boundary slot empty (slot_row: nslots entries), then launches k(a).
+  cudaError_t launch(const Args & a, uint32_t * slot_row, cudaStream_t s) const {
+    const cudaError_t e = nslots ? cudaMemsetAsync(slot_row, 0xff, nslots * sizeof(uint32_t), s) : cudaSuccess;
+    if (e != cudaSuccess) return e;
+    k<<<grid, kThreads, smem, s>>>(a);
+    spb200_count_launches(1);
+    return cudaGetLastError();
+  }
+};
+
+// The largest slot count of a run's launches: one slot buffer serves every mode.
+template <class Launch>
+unsigned long long max_slots(const Launch * ml, int N) {
+  unsigned long long n = 0;
+  for (int m = 0; m < N; ++m) n = std::max(n, ml[m].nslots);
+  return n;
+}
+
+// Grid of the elementwise kernels over rows x R entries.
+unsigned elementwise_grid(uint64_t rows, int R) {
+  return (unsigned)std::max<uint64_t>(std::min<uint64_t>((rows * R + kThreads - 1) / kThreads, 1184), 1);
+}
+
+// The walker arguments of one stream: its records and levels, the factors by level
+// (mats_by_mode[perm[l]]), ldm and R.
+TcArgs walk_args(const FiberStream & fs, const double * const * mats_by_mode, int ldm, int R) {
   const int N = fs.nmodes;
+  TcArgs a = {};
   a.rec = fs.rec;
   for (int l = 0; l < SPB200_MAXN - 2; ++l) a.up[l] = (l <= N - 3) ? fs.up[l] : nullptr;
   a.desc    = fs.desc;
   a.nrec    = fs.nrec;
   a.nchunks = static_cast<unsigned int>(fs.nchunks);
+  for (int l = 0; l < N; ++l) a.mats[l] = mats_by_mode[fs.perm[l]];
+  a.ldm = ldm;
+  a.R   = R;
+  return a;
 }
 
 // Launches a model-sum kernel (k(a) over the stream's records, the ring in dynamic shared memory)
 // on every resident CTA.
 cudaError_t launch_model_sum(void (*k)(TcArgs), const TcArgs & a, cudaStream_t s) {
   const size_t smem = tc_ring_bytes();
-  cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  if (e != cudaSuccess) return e;
-  int nb = 0;
-  e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k, kThreads, smem);
-  if (e != cudaSuccess) return e;
-  k<<<std::max(nb, 1) * num_sms(), kThreads, smem, s>>>(a);
+  const int grid = resident_grid(k, smem);
+  if (grid < 1) return cudaErrorInvalidConfiguration;
+  k<<<grid, kThreads, smem, s>>>(a);
   spb200_count_launches(1);
   return cudaGetLastError();
 }
@@ -295,6 +375,21 @@ bool factors_ok(int N, int R, int ldm, const void * const * d_factors) {
 }
 
 bool stream_fits(const FiberStream & fs) { return fs.nchunks <= 0xffffffffull; }
+
+// A whole ALLROOT tensor with 2..MAXN modes whose every mode m has a root stream with m at its
+// root that the walkers can index.
+bool root_streams_ok(const splatt_b200_tensor * t) {
+  if (!t || t->nmodes < 2 || t->nmodes > SPB200_MAXN || t->shard_count > 1 ||
+      t->layout != SPLATT_B200_LAYOUT_ALLROOT || t->streams.empty())
+    return false;
+  for (int m = 0; m < t->nmodes; ++m) {
+    const ModePlan & p = t->plan[m];
+    if (p.stream < 0 || p.stream >= (int)t->streams.size() || p.kind != SPB200_KIND_ROOT ||
+        t->streams[p.stream].perm[0] != m || !stream_fits(t->streams[p.stream]))
+      return false;
+  }
+  return true;
+}
 
 }  // namespace
 }  // namespace spb200
