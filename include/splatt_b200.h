@@ -693,6 +693,64 @@ int splatt_b200_cp_apr_device(splatt_b200_tensor const * t, int ncolumns, int ld
                               double * const * d_factors, double * lambda_out,
                               double * history, int * iterations_out, void * stream);
 
+/* Parameters of CP-APR by PDNR beyond options[NITER] and options[TOLERANCE]. */
+typedef struct {
+  int    max_inner;      /* lockstep Newton iterations per mode, >= 1 (default 10) */
+  int    max_backtrack;  /* trial steps of the line search, 1..8 (default 8) */
+  double mu0;            /* initial and smallest damping, > 0 (default 1e-5) */
+  double eps_active;     /* bound of the epsilon-active set, >= 0 (default 1e-8) */
+  double eps_div_zero;   /* floor of the model value in a division or a log, > 0 (default 1e-10) */
+} splatt_b200_pdnr_opts;
+
+/* Poisson CP decomposition by CP-APR with row-wise projected damped Newton steps (PDNR; Hansen,
+ * Plantenga & Kolda, Optim. Methods Softw. 2015).  Model, objective LL, start and outputs are
+ * those of splatt_b200_cp_apr_device; there is no shift.  One outer iteration runs, for
+ * n = 0 .. N-1:
+ *   1. B = A_n diag(lambda).
+ *   2. Every row i of B is its own problem: minimise
+ *        f_i(b) = sum_r b_r - sum_{x in X_i} v_x log(max(m_x(b), eps)),  m_x(b) = b . Pi_x,
+ *      X_i the stored x with i_n(x) = i and Pi_x the Hadamard product of the other modes' rows,
+ *      from b = B[i,:] with mu_i = mu0; g = 1 - sum_x (v_x / max(m_x, eps)) Pi_x and
+ *      H = sum_x (v_x / max(m_x, eps)^2) Pi_x Pi_x^T.  Up to max_inner lockstep iterations, every
+ *      row still active:
+ *      - kkt_i = max_r |min(b_r, g_r)|; if kkt_i < TOLERANCE the row stops and keeps b;
+ *      - eps_i = min(eps_active, ||b - max(b - g, 0)||_2); the active set is
+ *        A = {r : b_r <= eps_i and g_r > 0}, F the rest;
+ *      - d_A = -g_A, and (H_FF + mu_i I) d_F = -g_F by Cholesky; if a pivot is <= 0 or not
+ *        finite, d = -g for this iteration;
+ *      - trial points b_k = max(b + 2^-k d, 0), k = 0 .. max_backtrack-1; the smallest k with
+ *        f_i(b_k) <= f_i(b) + 1e-4 g^T (b_k - b) and f_i(b_k) <= f_i(b) is accepted, b <- b_k.
+ *        The change f_i(b_k) - f_i(b) is evaluated as
+ *        sum_r (b_k - b)_r - sum_x v_x log(max(m_x + delta_x, eps) / max(m_x, eps)),
+ *        delta_x = (b_k - b) . Pi_x, the log of the ratio by log1p(delta_x / m_x) where neither
+ *        value is floored, so a decrease stays visible near the row's minimum;
+ *      - if k = 0 was accepted mu_i <- max(mu_i / 3.5, mu0), else (a larger k, or none passed,
+ *        b unchanged) mu_i <- 3.5 mu_i.
+ *      The lockstep loop of a mode ends early when no row is active.
+ *   3. lambda = the column sums of B, A_n = B diag(1 / lambda) (a column with lambda_r = 0
+ *      becomes 0).
+ * Stops after options[NITER] outer iterations, or after one in which every row of every mode had
+ * kkt_i < TOLERANCE at its first evaluation.  sum_i f_i(B[i]) = -LL and the accept rule never
+ * raises an f_i, so LL does not decrease from mode to mode, up to rounding in the sums.
+ *   pdnr          NULL for the defaults (10, 8, 1e-5, 1e-8, 1e-10).
+ *   d_factors[m], lambda_out, iterations_out: as splatt_b200_cp_apr_device.
+ *   history       NULL, or 4 doubles per outer iteration run: LL after it, the largest
+ *                 last-computed kkt_i over all rows and modes, the lockstep iterations run summed
+ *                 over the modes, and the Newton steps attempted (a line search run, whether
+ *                 or not a trial point passed) summed over rows and modes.
+ * On untiled streams lambda, the factors and the history's last three columns are bitwise
+ * reproducible from run to run; on leaf-tiled streams the gradient, Hessian and line-search sums
+ * are added with atomics and may vary in the last bits.  Runs on t->device, enqueues on `stream`,
+ * synchronises it once per lockstep iteration (the count of rows that attempted a step) and once per
+ * outer iteration (the history).  VERBOSITY above NONE prints one line per outer iteration.
+ * Input rules: those of splatt_b200_cp_apr_device, and max_inner >= 1, 1 <= max_backtrack <= 8,
+ * mu0 > 0, eps_active >= 0 and eps > 0, all finite.  A violation returns SPLATT_ERROR_BADINPUT and
+ * the factors are left bit-identical. */
+int splatt_b200_cp_apr_pdnr_device(splatt_b200_tensor const * t, int ncolumns, int ldm,
+                                   double const * options, splatt_b200_pdnr_opts const * pdnr,
+                                   double * const * d_factors, double * lambda_out,
+                                   double * history, int * iterations_out, void * stream);
+
 /* TTMc, the kernel of Tucker: d_out = X_(mode) (kron_{m != mode} U_m), a dims[mode] x C_mode
  * row-major device matrix with leading dimension C_mode = prod_{m != mode} ranks[m], U_m =
  * columns [0, ranks[m]) of d_mats[m] (dims[m] x ldm, row-major).  Column order: the other modes

@@ -88,6 +88,11 @@ class AprOpts(C.Structure):
                 ("eps_div_zero", C.c_double)]
 
 
+class PdnrOpts(C.Structure):
+    _fields_ = [("max_inner", C.c_int), ("max_backtrack", C.c_int), ("mu0", C.c_double),
+                ("eps_active", C.c_double), ("eps_div_zero", C.c_double)]
+
+
 class TuckerOpts(C.Structure):
     _fields_ = [("max_power", C.c_int), ("svd_tol", C.c_double)]
 
@@ -114,7 +119,7 @@ EXPORTS = [
     "splatt_b200_cpd_nonneg_device", "splatt_b200_cpd_nonneg_device_f32",
     "splatt_b200_tensor_shard", "splatt_b200_mttkrp_multicast_sync",
     "splatt_b200_mttkrp_multicast_sync_columns", "splatt_b200_tensor_sse", "splatt_b200_tc_als_device",
-    "splatt_b200_cp_apr_device", "splatt_b200_ttmc", "splatt_b200_tucker_hooi_device",
+    "splatt_b200_cp_apr_device", "splatt_b200_cp_apr_pdnr_device", "splatt_b200_ttmc", "splatt_b200_tucker_hooi_device",
     "splatt_b200_multi_env_devices", "splatt_b200_multi_create", "splatt_b200_multi_free",
     "splatt_b200_multi_info", "splatt_b200_multi_mttkrp_host", "splatt_b200_multi_cpd_als",
     "splatt_b200_multi_last_ms", "splatt_b200_build_count", "splatt_b200_cache_clear",
@@ -238,6 +243,10 @@ def load() -> C.CDLL:
     lib.splatt_b200_cp_apr_device.argtypes = [C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_double),
                                               C.POINTER(AprOpts), vpp, val_p, val_p,
                                               C.POINTER(C.c_int), C.c_void_p]
+    lib.splatt_b200_cp_apr_pdnr_device.restype = C.c_int
+    lib.splatt_b200_cp_apr_pdnr_device.argtypes = [C.c_void_p, C.c_int, C.c_int,
+                                                   C.POINTER(C.c_double), C.POINTER(PdnrOpts), vpp,
+                                                   val_p, val_p, C.POINTER(C.c_int), C.c_void_p]
     lib.splatt_b200_ttmc.restype = C.c_int
     lib.splatt_b200_ttmc.argtypes = [C.c_void_p, C.c_int, C.POINTER(C.c_int), C.c_int, vpp, val_p,
                                      C.c_void_p]

@@ -548,6 +548,41 @@ class Tensor:
         _check(rc, "splatt_b200_cp_apr_device")
         return lam, [b[:, :rank] for b in bufs], hist[:its.value].copy(), its.value
 
+    def cp_apr_pdnr(self, rank: int, factors=None, *, niters: int = 50, tol: float = 1e-4,
+                    max_inner: int = 10, max_backtrack: int = 8, mu0: float = 1e-5,
+                    eps_active: float = 1e-8, eps: float = 1e-10, seed: int = 0,
+                    verbosity: int = 0, stream=None):
+        """Poisson CP decomposition by CP-APR with row-wise projected damped Newton steps
+        (PDNR, splatt_b200_cp_apr_pdnr_device): the model and objective of `cp_apr`, each mode's
+        rows solved as separate convex problems by up to `max_inner` Newton steps with a
+        `max_backtrack`-point projected line search, damping `mu0` and epsilon-active set
+        `eps_active`.  Needs what `cp_apr` needs; factors and seed as in `cp_apr`.  A row stops
+        when its KKT violation is below `tol`; the run stops after `niters` outer iterations or
+        after one in which every row stopped at its first evaluation.
+        Returns (lam (numpy float64[rank]), factors (CUDA views dims[m] x rank), history (numpy
+        float64 [iterations x 4] of (log-likelihood, largest last KKT violation, lockstep
+        iterations summed over the modes, Newton steps attempted summed over rows and modes)),
+        iterations)."""
+        import torch
+        self._check_factors(factors, [rank] * self.nmodes, torch.float64, "CP-APR")
+        ldm = rank + (rank & 1)
+        bufs = self._start_factors(factors, [rank] * self.nmodes, ldm, torch.float64, seed,
+                                   lambda v, g: v.uniform_(0.0, 1.0, generator=g))
+        o = default_opts()
+        o[A.OPTION_NITER] = niters
+        o[A.OPTION_TOLERANCE] = tol
+        o[A.OPTION_VERBOSITY] = verbosity
+        po = A.PdnrOpts(max_inner, max_backtrack, mu0, eps_active, eps)
+        s, ptrs = _launch_args(bufs, stream)
+        lam = np.zeros(rank)
+        hist = np.full((max(int(niters), 0), 4), np.nan)
+        its = C.c_int()
+        rc = self.lib.splatt_b200_cp_apr_pdnr_device(self.h, rank, ldm, _dptr(o), C.byref(po),
+                                                     ptrs, _dptr(lam), _dptr(hist), C.byref(its),
+                                                     C.c_void_p(s))
+        _check(rc, "splatt_b200_cp_apr_pdnr_device")
+        return lam, [b[:, :rank] for b in bufs], hist[:its.value].copy(), its.value
+
     def ttmc(self, mode: int, mats, out, ranks):
         """TTMc (splatt_b200_ttmc): out = X_(mode) times the Kronecker product of mats[m][:, :ranks[m]],
         m != mode, columns in mode order with the highest mode fastest.  mats: float64 CUDA tensors

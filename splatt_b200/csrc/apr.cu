@@ -210,6 +210,471 @@ __global__ void __launch_bounds__(kThreads, 3) k_apr_ll(const TcArgs a) {
   model_sum<N>(a, [eps](double s, double v, double x) { return fma(v, log(fmax(x, eps)), s); });
 }
 
+// ---- PDNR: projected damped Newton on the rows ----------------------------------------------------
+//
+// splatt_b200_cp_apr_pdnr_device (Hansen, Plantenga & Kolda, OMS 2015).  Row i of B = A_n diag(lambda)
+// minimises f_i(b) = sum_r b_r - sum_{x in X_i} v_x log(max(b . Pi_x, eps)) on its own, so one
+// lockstep iteration of mode n is:
+//   * k_pdnr_grad walks mode n's root stream like k_apr_phi and, for every row still to be
+//     evaluated (state 1), accumulates per record w Pi_x (w = v / max(m, eps)) and, with
+//     k_tc_update's pair-row accumulation, h h^T with h = (sqrt(v) / max(m, eps)) Pi_x: the
+//     Hessian.  A whole slice is finished in the warp where it closes (pdnr_step: g, kkt, the
+//     epsilon-active set, the reduced damped Cholesky solve, the direction); the first and last
+//     slice of a range go to boundary slots and k_pdnr_solve adds them in range order and runs
+//     pdnr_step.  k_pdnr_solve also serves the rows without records (g = 1, H = 0) and, on
+//     leaf-tiled streams, every row from its red.add-accumulated pack.
+//   * k_pdnr_ladder walks the stream again for the rows with a direction (state 2) and sums, for
+//     all kPdnrTrials trial points b_k = max(b + 2^-k d, 0) at once, v log(m_k / m) with
+//     m = b . Pi_x and m_k - m = (b_k - b) . Pi_x.  The eight dot products per record are reduced
+//     by a transposed butterfly (9 shuffles, lane group k ends with sum k) instead of 8 warp sums.
+//     Cut slices go through boundary slots and k_apr_combine, leaf-tiled pieces through red.add.
+//   * k_pdnr_accept, one thread per row: f(b_k) - f(b) = sum_r (b_k - b)_r - (ladder sum k), the
+//     smallest k that passes the Armijo and the decrease test, the damping, and the count of rows
+//     that attempted a step (the host reads it once per lockstep iteration).
+
+constexpr int    kPdnrTrials = 8;       // trial points the ladder scores (the largest max_backtrack)
+constexpr double kArmijo     = 1e-4;
+constexpr double kDamping    = 3.5;
+
+// Row states: 0 stopped (kkt < tol), 1 to be evaluated by the next gradient walk, 2 has a
+// direction for the ladder and the accept.
+struct PdnrArgs {
+  TcArgs          w;           // the walk: mats[0] = B, eps, packs / slot_row
+  double *        D;           // rows x ldm: the direction of every row in state 2
+  double *        G;           // rows x ldm: the gradient of every row in state 2
+  double *        lad;         // rows x kPdnrTrials: sum_x v log(m_k / m)
+  double *        kkt;         // rows: the last kkt of every row
+  const double *  mu;          // rows: the damping
+  int *           state;       // rows
+  unsigned char * mark;        // rows: 1 when the row has a record (set by every gradient walk)
+  double          tol, eps_active;
+};
+
+// doubles per warp of the gradient walk / solve workspace: the pack (2 NP + RT: the pair rows and
+// sum w Pi), h, b and the right-hand side / solution
+__host__ __device__ constexpr int pdnr_ws_doubles(int RT) { return 2 * tc_pairs(RT / 2) + 4 * RT; }
+__host__ __device__ constexpr size_t pdnr_tab_bytes(int RT) { return (sizeof(uint32_t) * tc_pairs(RT / 2) + 15) & ~size_t(15); }
+__host__ __device__ constexpr size_t pdnr_grad_smem(int RT) {
+  return tc_ring_bytes() + pdnr_tab_bytes(RT) + sizeof(double) * kWarps * pdnr_ws_doubles(RT);
+}
+__host__ __device__ constexpr int pdnr_minb(int RT) { return RT <= 32 ? 2 : 1; }
+
+// Trial point k of b along d: max(b + 2^-k d, 0).  The ladder and the accept use this one
+// expression, so both see bitwise the same point.
+__device__ __forceinline__ double pdnr_trial(double b, double d, int k) {
+  return fmax(fma(1.0 / static_cast<double>(1 << k), d, b), 0.0);
+}
+
+// One row's Newton step, one warp.  W: the row's pack (pair rows of H, then sum w Pi at
+// W + 2 tc_pairs(H)); bv, xv: R doubles of scratch each.  Computes g = 1 - sum w Pi and
+// kkt = max |min(b, g)|; stops the row when kkt < tol; else the epsilon-active set
+// A = {r: b_r <= min(eps_active, ||b - max(b - g, 0)||), g_r > 0}, d_A = -g_A and
+// (H_FF + mu I) d_F = -g_F by Cholesky over the free indices only (d = -g when a pivot is <= 0
+// or not finite), and stores d, g and state 2.  (The arguments are passed by value: a reference
+// to the kernel's parameters would copy them to the stack.)
+__device__ __noinline__ void pdnr_step(double * W, int R, int H, uint32_t row, const double * __restrict__ B,
+                                       double * __restrict__ D, double * __restrict__ G, int ldm,
+                                       double * __restrict__ kkt_out, const double * __restrict__ mu_in,
+                                       int * __restrict__ state, double tol, double eps_active,
+                                       double * bv, double * xv) {
+  const int lane = threadIdx.x & 31;
+  double *  g    = W + 2 * tc_pairs(H);
+  auto A = [&](int i, int j) -> double & { return W[2 * pair_base(i, H) + j - (i & ~1)]; };
+  const double * brow = B + static_cast<size_t>(row) * ldm;
+  double kkt = 0.0, e2 = 0.0;
+  for (int j = lane; j < R; j += 32) {
+    const double bj = brow[j], gj = 1.0 - g[j];
+    g[j] = gj;
+    bv[j] = bj;
+    kkt = fmax(kkt, fabs(fmin(bj, gj)));
+    const double t = bj - fmax(bj - gj, 0.0);
+    e2 = fma(t, t, e2);
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    kkt = fmax(kkt, __shfl_xor_sync(0xffffffffu, kkt, o));
+    e2 += __shfl_xor_sync(0xffffffffu, e2, o);
+  }
+  if (lane == 0) kkt_out[row] = kkt;
+  if (kkt < tol) {
+    if (lane == 0) state[row] = 0;
+    __syncwarp();
+    return;
+  }
+  const double ei = fmin(eps_active, sqrt(e2));
+  const unsigned lo = __ballot_sync(0xffffffffu, lane < R && bv[lane] <= ei && g[lane] > 0.0);
+  const unsigned hi = __ballot_sync(0xffffffffu, lane + 32 < R && bv[lane + 32] <= ei && g[lane + 32] > 0.0);
+  const unsigned long long act = lo | static_cast<unsigned long long>(hi) << 32;
+  auto free_ = [act](int j) { return !((act >> j) & 1ull); };
+  const double mu = mu_in[row];
+  for (int j = lane; j < R; j += 32) {
+    xv[j] = -g[j];
+    if (free_(j)) A(j, j) += mu;
+  }
+  __syncwarp();
+  bool ok = true;
+  for (int k = 0; k < R; ++k) {                // H_FF + mu I = U^T U over the free indices
+    if (!free_(k)) continue;
+    const double piv = A(k, k);
+    if (!(piv > 0.0 && piv <= 1.7976931348623157e308)) { ok = false; break; }
+    const double d = sqrt(piv);
+    __syncwarp();
+    const double inv = 1.0 / d;
+    for (int j = k + 1 + lane; j < R; j += 32)
+      if (free_(j)) A(k, j) *= inv;
+    if (lane == 0) A(k, k) = d;
+    __syncwarp();
+    for (int i = k + 1; i < R; ++i) {
+      if (!free_(i)) continue;
+      const double aki = A(k, i);
+      for (int j = i + lane; j < R; j += 32)
+        if (free_(j)) A(i, j) = fma(-aki, A(k, j), A(i, j));
+    }
+    __syncwarp();
+  }
+  __syncwarp();
+  if (ok) {
+    for (int k = 0; k < R; ++k) {              // U^T y = -g_F
+      if (!free_(k)) continue;
+      const double yk = xv[k] / A(k, k);
+      __syncwarp();
+      for (int j = k + 1 + lane; j < R; j += 32)
+        if (free_(j)) xv[j] = fma(-A(k, j), yk, xv[j]);
+      if (lane == 0) xv[k] = yk;
+      __syncwarp();
+    }
+    for (int k = R - 1; k >= 0; --k) {         // U d_F = y
+      if (!free_(k)) continue;
+      const double xk = xv[k] / A(k, k);
+      __syncwarp();
+      for (int i = lane; i < k; i += 32)
+        if (free_(i)) xv[i] = fma(-A(i, k), xk, xv[i]);
+      if (lane == 0) xv[k] = xk;
+      __syncwarp();
+    }
+  }
+  double * drow = D + static_cast<size_t>(row) * ldm;
+  double * grow = G + static_cast<size_t>(row) * ldm;
+  for (int j = lane; j < R; j += 32) {
+    drow[j] = ok ? xv[j] : -g[j];
+    grow[j] = g[j];
+  }
+  if (lane == 0) state[row] = 2;
+  __syncwarp();
+}
+
+// pdnr_step of row `row` with the pack at W
+__device__ __forceinline__ void pdnr_step(double * W, int H, uint32_t row, const PdnrArgs & p, double * bv,
+                                          double * xv) {
+  pdnr_step(W, p.w.R, H, row, p.w.mats[0], p.D, p.G, p.w.ldm, p.kkt, p.mu, p.state, p.tol, p.eps_active, bv, xv);
+}
+
+// Gradient and Hessian walk of the root mode of one stream (RT: the rank tier, the Hessian's
+// pair rows in registers at 16 and in per-warp shared memory at 32 / 64; ROWS: leaf-tiled
+// stream, every closed piece is added into its row's pack with red.add).
+template <int N, int RT, bool ROWS>
+__global__ void __launch_bounds__(kThreads, pdnr_minb(RT)) k_pdnr_grad(const PdnrArgs p) {
+  constexpr int  HM  = RT / 2;
+  constexpr int  S   = (tc_pairs(HM) + 31) / 32;   // pairs per lane
+  constexpr bool REG = (RT <= 16);
+  const TcArgs & a = p.w;
+  extern __shared__ __align__(128) unsigned char smem[];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int RP = a.R + (a.R & 1), H = RP / 2, NPr = tc_pairs(H), P = 2 * NPr + RP;
+  uint32_t * tab = reinterpret_cast<uint32_t *>(smem + tc_ring_bytes());
+  double *   ws  = reinterpret_cast<double *>(smem + tc_ring_bytes() + pdnr_tab_bytes(RT)) +
+                   warp * pdnr_ws_doubles(RT);
+  double2 *  W2  = reinterpret_cast<double2 *>(ws);
+  double *   hs  = ws + 2 * tc_pairs(HM) + RT;
+  double *   bv  = hs + RT;
+  double *   xv  = bv + RT;
+
+  // pair p -> (row i, first column j0): i in bits 0..15, j0 / 2 in bits 16..31
+  for (int i = warp; i < RP; i += kWarps)
+    for (int q = lane; q < H - i / 2; q += 32) tab[pair_base(i, H) + q] = uint32_t(i) | uint32_t(i / 2 + q) << 16;
+  for (int q = lane; q < P; q += 32) ws[q] = 0.0;
+  __syncthreads();
+
+  const bool act  = 2 * lane < a.R;
+  const bool hasy = 2 * lane + 1 < a.R;
+  double2    acc[REG ? S : 1];
+  uint32_t   ent[REG ? S : 1];
+  if constexpr (REG) {
+#pragma unroll
+    for (int k = 0; k < S; ++k) {
+      acc[k] = make_double2(0.0, 0.0);
+      ent[k] = (k * 32 + lane < NPr) ? tab[k * 32 + lane] : 0u;
+    }
+  }
+  double2 b    = make_double2(0.0, 0.0);
+  double2 gw   = make_double2(0.0, 0.0);
+  bool    open = true;    // the next record opens a slice
+  bool    live = false;   // the open slice's row is to be evaluated
+  bool    seen = false;   // this warp closed a slice already: later ones (but the last) are whole
+  const unsigned long long gwarp = static_cast<unsigned long long>(blockIdx.x) * kWarps + warp;
+
+  walk_range<N, 1, true>(a, smem, act, [&](double v, double2 h, bool close, uint32_t row, bool last) {
+    if (open) {
+      live = p.state[row] == 1;
+      if (live && act) b = reinterpret_cast<const double2 *>(a.mats[0] + static_cast<size_t>(row) * a.ldm)[lane];
+      if (!hasy) b.y = 0.0;
+      if (lane == 0) p.mark[row] = 1;
+      open = false;
+    }
+    if (live) {
+      if (!hasy) h.y = 0.0;                 // column R of an odd rank never feeds the result
+      double m = b.x * h.x;
+      m = fma(b.y, h.y, m);
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) m += __shfl_xor_sync(0xffffffffu, m, o);
+      const double mm = fmax(m, a.eps);
+      gw = vfma(v / mm, h, gw);
+      if (act) reinterpret_cast<double2 *>(hs)[lane] = vmul(sqrt(v) / mm, h);
+      __syncwarp();
+#pragma unroll
+      for (int k = 0; k < S; ++k) {
+        const int q = k * 32 + lane;
+        if (q < NPr) {
+          const uint32_t e  = REG ? ent[k] : tab[q];
+          const double   hi = hs[e & 0xffffu];
+          const double2  hj = reinterpret_cast<const double2 *>(hs)[e >> 16];
+          if constexpr (REG) acc[k] = vfma(hi, hj, acc[k]);
+          else W2[q] = vfma(hi, hj, W2[q]);
+        }
+      }
+      __syncwarp();                         // h is rewritten by the next record
+    }
+    if (!close) return;
+    open = true;
+    if (live) {
+      if constexpr (REG) {
+#pragma unroll
+        for (int k = 0; k < S; ++k) {
+          if (k * 32 + lane < NPr) W2[k * 32 + lane] = acc[k];
+          acc[k] = make_double2(0.0, 0.0);
+        }
+      }
+      if (act) reinterpret_cast<double2 *>(ws + 2 * NPr)[lane] = gw;
+      gw = make_double2(0.0, 0.0);
+      __syncwarp();
+      if constexpr (ROWS) {
+        double * dst = a.packs + static_cast<size_t>(row) * P;
+        for (int q = lane; q < P; q += 32) atomicAdd(dst + q, ws[q]);
+      } else if (!seen || last) {
+        const unsigned long long slot = 2 * gwarp + (seen ? 1 : 0);
+        double * dst = a.packs + slot * P;
+        for (int q = lane; q < P; q += 32) dst[q] = ws[q];
+        if (lane == 0) a.slot_row[slot] = row;
+      } else {
+        pdnr_step(ws, H, row, p, bv, xv);
+      }
+      __syncwarp();
+      for (int q = lane; q < P; q += 32) ws[q] = 0.0;
+      __syncwarp();
+    }
+    seen = true;
+  });
+}
+
+// The Newton step of the rows the gradient walk left: with slot_row, every row of the boundary
+// slots (the warp of a row's first slot adds all its slots, in range order), then every row in
+// state 1 without a record (g = 1, H = 0); without slot_row (leaf-tiled), every row in state 1
+// from its pack.
+template <int RT>
+__global__ void __launch_bounds__(kThreads) k_pdnr_solve(const PdnrArgs p, unsigned long long nslots,
+                                                         unsigned long long rows) {
+  extern __shared__ __align__(128) unsigned char smem[];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int RP = p.w.R + (p.w.R & 1), H = RP / 2, P = 2 * tc_pairs(H) + RP;
+  double *  ws = reinterpret_cast<double *>(smem) + warp * pdnr_ws_doubles(RT);
+  double *  bv = ws + 2 * tc_pairs(RT / 2) + 2 * RT;
+  double *  xv = bv + RT;
+  const uint32_t * slot_row = p.w.slot_row;
+  const unsigned long long TW = static_cast<unsigned long long>(gridDim.x) * kWarps;
+  const unsigned long long nitems = (slot_row ? nslots : 0) + rows;
+  for (unsigned long long s = static_cast<unsigned long long>(blockIdx.x) * kWarps + warp; s < nitems;
+       s += TW) {
+    uint32_t row;
+    if (slot_row && s < nslots) {
+      row = slot_row[s];
+      if (row == kEmptySlot) continue;
+      long long t = static_cast<long long>(s) - 1;
+      while (t >= 0 && slot_row[t] == kEmptySlot) --t;
+      if (t >= 0 && slot_row[t] == row) continue;          // not the row's first slot
+      for (int q = lane; q < P; q += 32) ws[q] = 0.0;
+      for (unsigned long long u = s; u < nslots; ++u) {
+        const uint32_t r2 = slot_row[u];
+        if (r2 == kEmptySlot) continue;
+        if (r2 != row) break;
+        const double * src = p.w.packs + u * P;
+        for (int q = lane; q < P; q += 32) ws[q] += src[q];
+      }
+    } else {
+      row = static_cast<uint32_t>(slot_row ? s - nslots : s);
+      if (p.state[row] != 1 || (slot_row && p.mark[row])) continue;
+      const double * src = p.w.packs + static_cast<size_t>(row) * P;
+      for (int q = lane; q < P; q += 32) ws[q] = slot_row ? 0.0 : src[q];
+    }
+    __syncwarp();
+    pdnr_step(ws, H, row, p, bv, xv);
+  }
+}
+
+// For every row with a direction, sum_x v log(max(m_k, eps) / max(m, eps)) over the trial points
+// k < kPdnrTrials into lad (ROWS: leaf-tiled stream, pieces added with red.add).
+template <int N, bool ROWS>
+__global__ void __launch_bounds__(kThreads, 2) k_pdnr_ladder(const PdnrArgs p) {
+  const TcArgs & a = p.w;
+  extern __shared__ __align__(128) unsigned char smem[];
+  const int  warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const bool act  = 2 * lane < a.R;
+  const bool hasy = 2 * lane + 1 < a.R;
+  // after the butterfly, lane group (lane & ~3) holds the sum of trial point k
+  const int  kown = ((lane >> 4) & 1) * 4 + ((lane >> 3) & 1) * 2 + ((lane >> 2) & 1);
+  const unsigned long long gwarp = static_cast<unsigned long long>(blockIdx.x) * kWarps + warp;
+  double2 b = make_double2(0.0, 0.0);
+  double2 t[kPdnrTrials];                  // b_k - b, the lane's two columns
+#pragma unroll
+  for (int k = 0; k < kPdnrTrials; ++k) t[k] = make_double2(0.0, 0.0);
+  double acc  = 0.0;
+  bool   open = true, live = false, seen = false;
+  walk_range<N, 1, true>(a, smem, act, [&](double v, double2 h, bool close, uint32_t row, bool last) {
+    if (open) {
+      live = p.state[row] == 2;
+      if (live) {
+        double2 d = make_double2(0.0, 0.0);
+        if (act) {
+          b = reinterpret_cast<const double2 *>(a.mats[0] + static_cast<size_t>(row) * a.ldm)[lane];
+          d = reinterpret_cast<const double2 *>(p.D + static_cast<size_t>(row) * a.ldm)[lane];
+        }
+        if (!hasy) b.y = d.y = 0.0;
+#pragma unroll
+        for (int k = 0; k < kPdnrTrials; ++k)
+          t[k] = make_double2(pdnr_trial(b.x, d.x, k) - b.x, pdnr_trial(b.y, d.y, k) - b.y);
+      }
+      open = false;
+    }
+    if (live) {
+      if (!hasy) h.y = 0.0;
+      double m = b.x * h.x;
+      m = fma(b.y, h.y, m);
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) m += __shfl_xor_sync(0xffffffffu, m, o);
+      double q[kPdnrTrials];
+#pragma unroll
+      for (int k = 0; k < kPdnrTrials; ++k) q[k] = fma(t[k].y, h.y, t[k].x * h.x);
+      // reduce-scatter: each round keeps half of the sums and sends the other half
+      {
+        const bool up = lane & 16;
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          const double send = up ? q[i] : q[i + 4], keep = up ? q[i + 4] : q[i];
+          q[i] = keep + __shfl_xor_sync(0xffffffffu, send, 16);
+        }
+      }
+      {
+        const bool up = lane & 8;
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          const double send = up ? q[i] : q[i + 2], keep = up ? q[i + 2] : q[i];
+          q[i] = keep + __shfl_xor_sync(0xffffffffu, send, 8);
+        }
+      }
+      {
+        const bool up = lane & 4;
+        const double send = up ? q[0] : q[1], keep = up ? q[1] : q[0];
+        q[0] = keep + __shfl_xor_sync(0xffffffffu, send, 4);
+      }
+      q[0] += __shfl_xor_sync(0xffffffffu, q[0], 2);
+      q[0] += __shfl_xor_sync(0xffffffffu, q[0], 1);
+      const double mk = m + q[0];
+      const double lr = (m >= a.eps && mk >= a.eps) ? log1p(q[0] / m) : log(fmax(mk, a.eps)) - log(fmax(m, a.eps));
+      acc = fma(v, lr, acc);
+    }
+    if (!close) return;
+    open = true;
+    if (live && (lane & 3) == 0) {
+      if constexpr (ROWS) {
+        atomicAdd(p.lad + static_cast<size_t>(row) * kPdnrTrials + kown, acc);
+      } else if (!seen || last) {
+        const unsigned long long slot = 2 * gwarp + (seen ? 1 : 0);
+        a.packs[slot * kPdnrTrials + kown] = acc;
+        if (lane == 0) a.slot_row[slot] = row;
+      } else {
+        p.lad[static_cast<size_t>(row) * kPdnrTrials + kown] = acc;
+      }
+    }
+    acc  = 0.0;
+    seen = true;
+  });
+}
+
+// The line search's decision for every row with a direction (one thread per row): the smallest
+// k < K with df_k <= 1e-4 g.(b_k - b) and df_k <= 0, df_k = sum_r (b_k - b)_r - lad[k]; b <- b_k
+// and the damping; the row goes back to state 1 and is counted into *count.
+__global__ void __launch_bounds__(kThreads) k_pdnr_accept(double * __restrict__ B, const double * __restrict__ D,
+                                                          const double * __restrict__ G,
+                                                          const double * __restrict__ lad, double * __restrict__ mu,
+                                                          int * __restrict__ state, unsigned long long rows, int R,
+                                                          int ldm, int K, double mu0, int * count) {
+  int n = 0;
+  for (unsigned long long i = blockIdx.x * static_cast<unsigned long long>(blockDim.x) + threadIdx.x; i < rows;
+       i += static_cast<unsigned long long>(gridDim.x) * blockDim.x) {
+    if (state[i] != 2) continue;
+    double * b = B + i * ldm;
+    const double * d = D + i * ldm;
+    const double * g = G + i * ldm;
+    double ds[kPdnrTrials], gd[kPdnrTrials];
+#pragma unroll
+    for (int k = 0; k < kPdnrTrials; ++k) ds[k] = gd[k] = 0.0;
+    for (int r = 0; r < R; ++r) {
+      const double br = b[r], dr = d[r], gr = g[r];
+#pragma unroll
+      for (int k = 0; k < kPdnrTrials; ++k) {
+        const double s = pdnr_trial(br, dr, k) - br;
+        ds[k] += s;
+        gd[k] = fma(gr, s, gd[k]);
+      }
+    }
+    int acc = -1;
+#pragma unroll
+    for (int k = 0; k < kPdnrTrials; ++k) {
+      const double df = ds[k] - lad[i * kPdnrTrials + k];
+      if (acc < 0 && k < K && df <= kArmijo * gd[k] && df <= 0.0) acc = k;
+    }
+    if (acc >= 0)
+      for (int r = 0; r < R; ++r) b[r] = pdnr_trial(b[r], d[r], acc);
+    mu[i] = acc == 0 ? fmax(mu[i] / kDamping, mu0) : mu[i] * kDamping;
+    state[i] = 1;
+    ++n;
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) n += __shfl_xor_sync(0xffffffffu, n, o);
+  if ((threadIdx.x & 31) == 0 && n) atomicAdd(count, n);
+}
+
+// Every row of a mode: state 1 (to be evaluated) and damping mu0.
+__global__ void __launch_bounds__(kThreads) k_pdnr_init(double * __restrict__ mu, int * __restrict__ state,
+                                                        unsigned long long rows, double mu0) {
+  for (unsigned long long i = blockIdx.x * static_cast<unsigned long long>(blockDim.x) + threadIdx.x; i < rows;
+       i += static_cast<unsigned long long>(gridDim.x) * blockDim.x) {
+    mu[i] = mu0;
+    state[i] = 1;
+  }
+}
+
+// *bits = max(*bits, max of kkt[0..rows)) on the bit patterns of nonnegative doubles
+__global__ void __launch_bounds__(kThreads) k_pdnr_kktmax(const double * __restrict__ kkt, unsigned long long rows,
+                                                          unsigned long long * bits) {
+  double m = 0.0;
+  for (unsigned long long i = blockIdx.x * static_cast<unsigned long long>(blockDim.x) + threadIdx.x; i < rows;
+       i += static_cast<unsigned long long>(gridDim.x) * blockDim.x)
+    m = fmax(m, kkt[i]);
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) m = fmax(m, __shfl_xor_sync(0xffffffffu, m, o));
+  if ((threadIdx.x & 31) == 0) atomicMax(bits, static_cast<unsigned long long>(__double_as_longlong(m)));
+}
+
 #undef APR_FOR_ENTRIES
 
 // ---- host side ---------------------------------------------------------------------------------
@@ -240,6 +705,105 @@ struct AprBuffers {
     for (double * p : phi) cudaFree(p);
   }
 };
+
+
+// The extra device buffers of one PDNR run (B, the slots, lambda, the sums and the flags are
+// AprBuffers').
+struct PdnrBuffers : AprBuffers {
+  double *   D = nullptr;                      // max dims x ldm: directions
+  double *   G = nullptr;                      // max dims x ldm: gradients
+  double *   lad = nullptr;                    // max dims x kPdnrTrials: ladder sums
+  double *   kkt_row = nullptr;                // max dims
+  double *   mu = nullptr;                     // max dims
+  int *      state = nullptr;                  // max dims
+  int *      count = nullptr;                  // one int: rows with a step
+  unsigned char * mark[SPB200_MAXN] = {nullptr};   // dims[m]: the row has a record
+  ~PdnrBuffers() {
+    cudaFree(D); cudaFree(G); cudaFree(lad); cudaFree(kkt_row); cudaFree(mu); cudaFree(state); cudaFree(count);
+    for (unsigned char * p : mark) cudaFree(p);
+  }
+};
+
+// The gradient walk of (N, tier, rows mode).
+template <int N>
+void (*pdnr_grad_kernel(int RT, bool rows))(PdnrArgs) {
+  if (RT == 16) return rows ? k_pdnr_grad<N, 16, true> : k_pdnr_grad<N, 16, false>;
+  if (RT == 32) return rows ? k_pdnr_grad<N, 32, true> : k_pdnr_grad<N, 32, false>;
+  return rows ? k_pdnr_grad<N, 64, true> : k_pdnr_grad<N, 64, false>;
+}
+
+// k_pdnr_solve over nslots boundary slots (p.w.slot_row set) and the rows of the mode.
+cudaError_t launch_pdnr_solve(const PdnrArgs & p, unsigned long long nslots, uint64_t rows, cudaStream_t s) {
+  const int RT = rank_tier(p.w.R);
+  const size_t smem = sizeof(double) * kWarps * pdnr_ws_doubles(RT);
+  void (*k)(const PdnrArgs, unsigned long long, unsigned long long) =
+      RT == 16 ? k_pdnr_solve<16> : (RT == 32 ? k_pdnr_solve<32> : k_pdnr_solve<64>);
+  cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  if (e != cudaSuccess) return e;
+  k<<<combine_grid((p.w.slot_row ? nslots : 0) + rows), kThreads, smem, s>>>(p, nslots, rows);
+  spb200_count_launches(1);
+  return cudaGetLastError();
+}
+
+// The start of both CP-APR solvers.  Checks the input rules on the device (tensor values and start
+// entries finite and >= 0, every start column with a positive sum), then divides every start
+// column of d_factors by its sum s_{m,r} and sets lambda_r = prod_m s_{m,r} (lam: RP host doubles,
+// also copied to b.lam).  Uses b.bad, b.sums, b.colsum_part and b.lam.  A violated rule returns
+// SPLATT_ERROR_BADINPUT before anything is written.
+int apr_start(const splatt_b200_tensor * t, int R, int ldm, double * const * d_factors, AprBuffers & b,
+              std::vector<double> & lam, cudaStream_t s, const char * name) {
+  const int N = t->nmodes, RP = R + (R & 1);
+  const FiberStream & fs0 = t->streams[0];
+  bool ok = cudaMemsetAsync(b.bad, 0, sizeof(int), s) == cudaSuccess &&
+            cudaMemsetAsync(b.sums, 0, (size_t)N * RP * sizeof(double), s) == cudaSuccess;
+  if (ok && fs0.nrec) {
+    // the records' values: the first double of every 16-byte record
+    k_apr_check<<<elementwise_grid(fs0.nrec, 1), kThreads, 0, s>>>(reinterpret_cast<const double *>(fs0.rec),
+                                                                   fs0.nrec, 1, 2, b.bad);
+    spb200_count_launches(1);
+  }
+  for (int m = 0; ok && m < N; ++m) {
+    k_apr_check<<<elementwise_grid(t->dims[m], R), kThreads, 0, s>>>(d_factors[m], t->dims[m], R, ldm, b.bad);
+    spb200_count_launches(1);
+    launch_colsum(d_factors[m], t->dims[m], R, ldm, b.colsum_part, b.sums + (size_t)m * RP, s);
+  }
+  std::vector<double> hs((size_t)N * RP, 0.0);
+  int hbad = 1;
+  ok = ok && cudaGetLastError() == cudaSuccess &&
+       cudaMemcpyAsync(hs.data(), b.sums, hs.size() * sizeof(double), cudaMemcpyDeviceToHost, s) == cudaSuccess &&
+       cudaMemcpyAsync(&hbad, b.bad, sizeof(int), cudaMemcpyDeviceToHost, s) == cudaSuccess &&
+       cudaStreamSynchronize(s) == cudaSuccess;
+  if (!ok) {
+    fprintf(stderr, "SPLATT: %s failed (%s)\n", name, cudaGetErrorString(cudaGetLastError()));
+    return SPLATT_ERROR_BADINPUT;
+  }
+  for (int m = 0; m < N && !hbad; ++m)
+    for (int r = 0; r < R; ++r)
+      if (!(std::isfinite(hs[(size_t)m * RP + r]) && hs[(size_t)m * RP + r] > 0.0)) hbad = 1;
+  if (hbad) {
+    fprintf(stderr, "SPLATT: %s: a tensor value or start entry is negative or not finite, or a start column "
+                    "sums to 0\n", name);
+    return SPLATT_ERROR_BADINPUT;
+  }
+
+  // start: every column divided by its sum, lambda_r = prod_m s_{m,r}
+  lam.assign(RP, 0.0);
+  for (int r = 0; r < R; ++r) {
+    lam[r] = 1.0;
+    for (int m = 0; m < N; ++m) lam[r] *= hs[(size_t)m * RP + r];
+  }
+  ok = cudaMemcpyAsync(b.lam, lam.data(), RP * sizeof(double), cudaMemcpyHostToDevice, s) == cudaSuccess;
+  for (int m = 0; ok && m < N; ++m) {
+    k_apr_normalize<<<elementwise_grid(t->dims[m], R), kThreads, 0, s>>>(d_factors[m], b.sums + (size_t)m * RP,
+                                                                         d_factors[m], t->dims[m], R, ldm);
+    spb200_count_launches(1);
+  }
+  if (!ok) {
+    fprintf(stderr, "SPLATT: %s failed (%s)\n", name, cudaGetErrorString(cudaGetLastError()));
+    return SPLATT_ERROR_BADINPUT;
+  }
+  return SPLATT_SUCCESS;
+}
 
 }  // namespace
 }  // namespace spb200
@@ -303,54 +867,13 @@ extern "C" int splatt_b200_cp_apr_device(splatt_b200_tensor const * t, int ncolu
     return SPLATT_ERROR_NOMEMORY;
   }
 
-  // input rules on the device: values and start entries finite and >= 0, start columns sum > 0
+  std::vector<double> lam;
+  const int rc = apr_start(t, R, ldm, d_factors, b, lam, s, "splatt_b200_cp_apr_device");
+  if (rc != SPLATT_SUCCESS) return rc;
   const FiberStream & fs0 = t->streams[0];
-  ok = cudaMemsetAsync(b.bad, 0, sizeof(int), s) == cudaSuccess &&
-       cudaMemsetAsync(b.sums, 0, (size_t)N * RP * sizeof(double), s) == cudaSuccess;
-  if (ok && fs0.nrec) {
-    // the records' values: the first double of every 16-byte record
-    k_apr_check<<<elementwise_grid(fs0.nrec, 1), kThreads, 0, s>>>(reinterpret_cast<const double *>(fs0.rec),
-                                                                   fs0.nrec, 1, 2, b.bad);
-    spb200_count_launches(1);
-  }
-  for (int m = 0; ok && m < N; ++m) {
-    k_apr_check<<<elementwise_grid(t->dims[m], R), kThreads, 0, s>>>(d_factors[m], t->dims[m], R, ldm, b.bad);
-    spb200_count_launches(1);
-    launch_colsum(d_factors[m], t->dims[m], R, ldm, b.colsum_part, b.sums + (size_t)m * RP, s);
-  }
-  std::vector<double> hs((size_t)N * RP, 0.0);
-  int hbad = 1;
-  ok = ok && cudaGetLastError() == cudaSuccess &&
-       cudaMemcpyAsync(hs.data(), b.sums, hs.size() * sizeof(double), cudaMemcpyDeviceToHost, s) == cudaSuccess &&
-       cudaMemcpyAsync(&hbad, b.bad, sizeof(int), cudaMemcpyDeviceToHost, s) == cudaSuccess &&
-       cudaStreamSynchronize(s) == cudaSuccess;
-  if (!ok) {
-    fprintf(stderr, "SPLATT: splatt_b200_cp_apr_device failed (%s)\n", cudaGetErrorString(cudaGetLastError()));
-    return SPLATT_ERROR_BADINPUT;
-  }
-  for (int m = 0; m < N && !hbad; ++m)
-    for (int r = 0; r < R; ++r)
-      if (!(std::isfinite(hs[(size_t)m * RP + r]) && hs[(size_t)m * RP + r] > 0.0)) hbad = 1;
-  if (hbad) {
-    fprintf(stderr, "SPLATT: splatt_b200_cp_apr_device: a tensor value or start entry is negative or not "
-                    "finite, or a start column sums to 0\n");
-    return SPLATT_ERROR_BADINPUT;
-  }
-
-  // start: every column divided by its sum, lambda_r = prod_m s_{m,r}
-  std::vector<double> lam(RP, 0.0);
-  for (int r = 0; r < R; ++r) {
-    lam[r] = 1.0;
-    for (int m = 0; m < N; ++m) lam[r] *= hs[(size_t)m * RP + r];
-  }
-  ok = cudaMemcpyAsync(b.lam, lam.data(), RP * sizeof(double), cudaMemcpyHostToDevice, s) == cudaSuccess &&
-       cudaMemsetAsync(b.B, 0, max_dim * ldm * sizeof(double), s) == cudaSuccess;
-  for (int m = 0; ok && m < N; ++m) {
-    k_apr_normalize<<<elementwise_grid(t->dims[m], R), kThreads, 0, s>>>(d_factors[m], b.sums + (size_t)m * RP,
-                                                                         d_factors[m], t->dims[m], R, ldm);
-    spb200_count_launches(1);
+  ok = cudaMemsetAsync(b.B, 0, max_dim * ldm * sizeof(double), s) == cudaSuccess;
+  for (int m = 0; ok && m < N; ++m)
     ok = cudaMemsetAsync(b.phi[m], 0, t->dims[m] * ldm * sizeof(double), s) == cudaSuccess;
-  }
 
   uint64_t its = 0;
   auto t0 = std::chrono::steady_clock::now();
@@ -433,6 +956,188 @@ extern "C" int splatt_b200_cp_apr_device(splatt_b200_tensor const * t, int ncolu
   }
   if (!ok) {
     fprintf(stderr, "SPLATT: splatt_b200_cp_apr_device failed (%s)\n", cudaGetErrorString(cudaGetLastError()));
+    cudaStreamSynchronize(s);
+    return SPLATT_ERROR_BADINPUT;
+  }
+  std::copy(lam.begin(), lam.begin() + R, lambda_out);
+  if (iterations_out) *iterations_out = (int)its;
+  return SPLATT_SUCCESS;
+}
+
+extern "C" int splatt_b200_cp_apr_pdnr_device(splatt_b200_tensor const * t, int ncolumns, int ldm,
+                                              double const * options, splatt_b200_pdnr_opts const * pdnr,
+                                              double * const * d_factors, double * lambda_out,
+                                              double * history, int * iterations_out, void * stream) {
+  static const char * name = "splatt_b200_cp_apr_pdnr_device";
+  const int R = ncolumns;
+  const splatt_b200_pdnr_opts o = pdnr ? *pdnr : splatt_b200_pdnr_opts{10, 8, 1e-5, 1e-8, 1e-10};
+  const double tol = options ? options[SPLATT_OPTION_TOLERANCE] : 0.0;
+  const double niter = options ? options[SPLATT_OPTION_NITER] : 0.0;
+  auto nonneg = [](double x) { return std::isfinite(x) && x >= 0.0; };
+  auto positive = [](double x) { return std::isfinite(x) && x > 0.0; };
+  bool bad = !root_streams_ok(t) || !options || !lambda_out ||
+             !factors_ok(t->nmodes, R, ldm, reinterpret_cast<const void * const *>(d_factors)) ||
+             o.max_inner < 1 || o.max_backtrack < 1 || o.max_backtrack > kPdnrTrials || !positive(o.mu0) ||
+             !nonneg(o.eps_active) || !positive(o.eps_div_zero) || !nonneg(tol) ||
+             !(niter >= 0.0 && niter <= 2147483647.0);
+  if (bad) {
+    fprintf(stderr, "SPLATT: %s: bad arguments\n", name);
+    return SPLATT_ERROR_BADINPUT;
+  }
+  DeviceGuard g(t->device);
+  if (!g.ok) return SPLATT_ERROR_BADINPUT;
+  const int N = t->nmodes;
+  const int RP = R + (R & 1), H = RP / 2;
+  const size_t P = 2 * (size_t)H * (H + 1) + RP;             // doubles of a gradient pack
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const uint64_t niters = (uint64_t)niter;
+  const int verbosity = (int)options[SPLATT_OPTION_VERBOSITY];
+
+  // per mode the gradient walk and the ladder walk; one pack buffer serves the largest need
+  // (boundary slots of either walk, or a pack per row on a leaf-tiled stream)
+  const int RT = rank_tier(R);
+  WalkLaunch<PdnrArgs> gl[SPB200_MAXN], ll[SPB200_MAXN];
+  uint64_t max_dim = 1;
+  size_t max_pack = 1;
+  for (int m = 0; m < N; ++m) {
+    const bool rows = t->streams[t->plan[m].stream].ktile_rows > 0;
+    auto lad = [rows](auto n) { return rows ? k_pdnr_ladder<n.value, true> : k_pdnr_ladder<n.value, false>; };
+    if (!gl[m].configure(with_nmodes(N, [&](auto n) { return pdnr_grad_kernel<n.value>(RT, rows); }),
+                         pdnr_grad_smem(RT), rows) ||
+        !ll[m].configure(with_nmodes(N, lad), tc_ring_bytes(), rows)) {
+      fprintf(stderr, "SPLATT: %s: cannot configure the walks (%s)\n", name, cudaGetErrorString(cudaGetLastError()));
+      return SPLATT_ERROR_BADINPUT;
+    }
+    max_dim = std::max<uint64_t>(max_dim, t->dims[m]);
+    max_pack = std::max<size_t>({max_pack, (rows ? t->dims[m] : gl[m].nslots) * P, ll[m].nslots * kPdnrTrials});
+  }
+  const unsigned long long max_slot = std::max({max_slots(gl, N), max_slots(ll, N), 1ull});
+  PdnrBuffers b;
+  bool ok = cudaMalloc(&b.B, max_dim * ldm * sizeof(double)) == cudaSuccess &&
+            cudaMalloc(&b.D, max_dim * ldm * sizeof(double)) == cudaSuccess &&
+            cudaMalloc(&b.G, max_dim * ldm * sizeof(double)) == cudaSuccess &&
+            cudaMalloc(&b.lad, max_dim * kPdnrTrials * sizeof(double)) == cudaSuccess &&
+            cudaMalloc(&b.kkt_row, max_dim * sizeof(double)) == cudaSuccess &&
+            cudaMalloc(&b.mu, max_dim * sizeof(double)) == cudaSuccess &&
+            cudaMalloc(&b.state, max_dim * sizeof(int)) == cudaSuccess &&
+            cudaMalloc(&b.count, sizeof(int)) == cudaSuccess &&
+            cudaMalloc(&b.packs, max_pack * sizeof(double)) == cudaSuccess &&
+            cudaMalloc(&b.slot_row, max_slot * sizeof(uint32_t)) == cudaSuccess &&
+            cudaMalloc(&b.lam, RP * sizeof(double)) == cudaSuccess &&
+            cudaMalloc(&b.sums, (size_t)N * RP * sizeof(double)) == cudaSuccess &&
+            cudaMalloc(&b.ll, sizeof(double)) == cudaSuccess &&
+            cudaMalloc(&b.kkt, sizeof(unsigned long long)) == cudaSuccess &&
+            cudaMalloc(&b.bad, sizeof(int)) == cudaSuccess &&
+            cudaMalloc(&b.colsum_part, kColsumCtas * 64 * sizeof(double)) == cudaSuccess;
+  for (int m = 0; ok && m < N; ++m)
+    ok = cudaMalloc(&b.mark[m], std::max<uint64_t>(t->dims[m], 1)) == cudaSuccess;
+  if (!ok) {
+    cudaGetLastError();
+    return SPLATT_ERROR_NOMEMORY;
+  }
+
+  std::vector<double> lam;
+  const int rc = apr_start(t, R, ldm, d_factors, b, lam, s, name);
+  if (rc != SPLATT_SUCCESS) return rc;
+  const FiberStream & fs0 = t->streams[0];
+  ok = cudaMemsetAsync(b.B, 0, max_dim * ldm * sizeof(double), s) == cudaSuccess;
+  for (int m = 0; ok && m < N; ++m) ok = cudaMemsetAsync(b.mark[m], 0, t->dims[m], s) == cudaSuccess;
+
+  uint64_t its = 0;
+  auto t0 = std::chrono::steady_clock::now();
+  for (uint64_t it = 0; ok && it < niters; ++it) {
+    if (verbosity > SPLATT_VERBOSITY_NONE) t0 = std::chrono::steady_clock::now();
+    bool converged = true;
+    long long lockstep = 0, steps = 0;
+    ok = cudaMemsetAsync(b.kkt, 0, sizeof(unsigned long long), s) == cudaSuccess;
+    for (int n = 0; ok && n < N; ++n) {
+      const FiberStream & fs = t->streams[t->plan[n].stream];
+      const WalkLaunch<PdnrArgs> & GL = gl[n];
+      const WalkLaunch<PdnrArgs> & LL = ll[n];
+      const uint64_t rows = t->dims[n];
+      const unsigned eg = elementwise_grid(rows, R);
+      // B = A_n diag(lambda) (no shift: A_n stands in for the unread Phi)
+      k_apr_scale<<<eg, kThreads, 0, s>>>(d_factors[n], d_factors[n], b.lam, b.B, rows, R, ldm, 0.0, 0.0, 0);
+      k_pdnr_init<<<elementwise_grid(rows, 1), kThreads, 0, s>>>(b.mu, b.state, rows, o.mu0);
+      spb200_count_launches(2);
+      PdnrArgs p = {};
+      p.w = walk_args(fs, d_factors, ldm, R);
+      p.w.mats[0] = b.B;
+      p.w.eps = o.eps_div_zero;
+      p.w.packs = b.packs;
+      p.w.slot_row = GL.rows ? nullptr : b.slot_row;
+      p.D = b.D; p.G = b.G; p.lad = b.lad; p.kkt = b.kkt_row; p.mu = b.mu; p.state = b.state;
+      p.mark = b.mark[n];
+      p.tol = tol; p.eps_active = o.eps_active;
+      for (int l = 0; ok && l < o.max_inner; ++l) {
+        // gradient, Hessian and direction of every row still to be evaluated
+        if (GL.rows) ok = cudaMemsetAsync(b.packs, 0, rows * P * sizeof(double), s) == cudaSuccess;
+        if (ok && fs.nrec) ok = GL.launch(p, b.slot_row, s) == cudaSuccess;
+        ok = ok && launch_pdnr_solve(p, GL.nslots, rows, s) == cudaSuccess;
+        // the ladder's sums and the line search's decision
+        ok = ok && cudaMemsetAsync(b.lad, 0, rows * kPdnrTrials * sizeof(double), s) == cudaSuccess &&
+             cudaMemsetAsync(b.count, 0, sizeof(int), s) == cudaSuccess;
+        if (ok && fs.nrec) {
+          ok = LL.launch(p, b.slot_row, s) == cudaSuccess;
+          if (ok && !LL.rows) {
+            k_apr_combine<<<combine_grid(LL.nslots), kThreads, 0, s>>>(b.packs, b.slot_row, LL.nslots, kPdnrTrials,
+                                                                       kPdnrTrials, b.lad);
+            spb200_count_launches(1);
+          }
+        }
+        k_pdnr_accept<<<elementwise_grid(rows, 1), kThreads, 0, s>>>(b.B, b.D, b.G, b.lad, b.mu, b.state, rows, R,
+                                                                     ldm, o.max_backtrack, o.mu0, b.count);
+        spb200_count_launches(1);
+        int cnt = 0;
+        ok = ok && cudaGetLastError() == cudaSuccess &&
+             cudaMemcpyAsync(&cnt, b.count, sizeof(int), cudaMemcpyDeviceToHost, s) == cudaSuccess &&
+             cudaStreamSynchronize(s) == cudaSuccess;
+        if (!ok) break;
+        ++lockstep;
+        steps += cnt;
+        if (cnt && l == 0) converged = false;
+        if (!cnt) break;
+      }
+      if (!ok) break;
+      k_pdnr_kktmax<<<elementwise_grid(rows, 1), kThreads, 0, s>>>(b.kkt_row, rows, b.kkt);
+      spb200_count_launches(1);
+      launch_colsum(b.B, rows, R, ldm, b.colsum_part, b.lam, s);
+      k_apr_normalize<<<eg, kThreads, 0, s>>>(b.B, b.lam, d_factors[n], rows, R, ldm);
+      spb200_count_launches(1);
+    }
+    if (!ok) break;
+    // log-likelihood of the iteration's model, lambda and the largest kkt, read back once
+    double ll = 0.0, kkt_max = 0.0;
+    unsigned long long bits = 0;
+    ok = cudaMemsetAsync(b.ll, 0, sizeof(double), s) == cudaSuccess;
+    if (ok && fs0.nrec) {
+      TcArgs a = walk_args(fs0, d_factors, ldm, R);
+      a.lambda = b.lam; a.sse = b.ll; a.eps = o.eps_div_zero;
+      ok = launch_model_sum(with_nmodes(N, [](auto n) { return k_apr_ll<n.value>; }), a, s) == cudaSuccess;
+    }
+    ok = ok && cudaMemcpyAsync(&ll, b.ll, sizeof(double), cudaMemcpyDeviceToHost, s) == cudaSuccess &&
+         cudaMemcpyAsync(lam.data(), b.lam, RP * sizeof(double), cudaMemcpyDeviceToHost, s) == cudaSuccess &&
+         cudaMemcpyAsync(&bits, b.kkt, sizeof(bits), cudaMemcpyDeviceToHost, s) == cudaSuccess &&
+         cudaStreamSynchronize(s) == cudaSuccess;
+    if (!ok) break;
+    std::memcpy(&kkt_max, &bits, sizeof(kkt_max));
+    for (int r = 0; r < R; ++r) ll -= lam[r];
+    if (history) {
+      history[4 * it] = ll;
+      history[4 * it + 1] = kkt_max;
+      history[4 * it + 2] = (double)lockstep;
+      history[4 * it + 3] = (double)steps;
+    }
+    its = it + 1;
+    if (verbosity > SPLATT_VERBOSITY_NONE) {
+      const double sec = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
+      printf("  its = %3llu (%0.3fs)  log-likelihood = %0.10e  kkt = %0.3e  lockstep = %lld  steps = %lld\n",
+             (unsigned long long)its, sec, ll, kkt_max, lockstep, steps);
+    }
+    if (converged) break;
+  }
+  if (!ok) {
+    fprintf(stderr, "SPLATT: %s failed (%s)\n", name, cudaGetErrorString(cudaGetLastError()));
     cudaStreamSynchronize(s);
     return SPLATT_ERROR_BADINPUT;
   }

@@ -37,12 +37,6 @@
 namespace spb200 {
 namespace {
 
-__host__ __device__ constexpr int tc_pairs(int H) { return H * (H + 1); }
-// pairs stored before pair row i (H = RP / 2): sum over i' < i of (H - i'/2)
-__device__ __forceinline__ int pair_base(int i, int H) {
-  const int q = i >> 1;
-  return i * H - ((i & 1) ? q * q : q * (q - 1));
-}
 // doubles per warp of the row-update / solve workspace: the pack (2 NP + RT) and h (RT)
 __host__ __device__ constexpr int tc_ws_doubles(int RT) { return 2 * tc_pairs(RT / 2) + 2 * RT; }
 __host__ __device__ constexpr size_t tc_tab_bytes(int RT) { return (sizeof(uint32_t) * tc_pairs(RT / 2) + 15) & ~size_t(15); }
@@ -250,8 +244,6 @@ __global__ void __launch_bounds__(kThreads) k_tc_sumsq(const double * __restrict
 }
 
 // ---- host side ---------------------------------------------------------------------------------
-
-int rank_tier(int R) { return R <= 16 ? 16 : (R <= 32 ? 32 : 64); }
 
 // The row-update kernel of (N, tier, rows mode).
 template <int N>

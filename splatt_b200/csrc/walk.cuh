@@ -32,6 +32,16 @@ struct TcArgs {
 
 __host__ __device__ constexpr size_t tc_ring_bytes() { return smem_bytes(kStages, false, 1, 0, 0); }
 
+// The upper triangle of an R x R matrix as "pair rows" (completion's row update, CP-APR's PDNR
+// Hessian): row i holds the column pairs (2q, 2q+1) for q = i/2 .. H - 1 (H = RP / 2, RP = R
+// rounded up to even), so every update is one double2 FMA; tc_pairs(H) pairs in all.
+__host__ __device__ constexpr int tc_pairs(int H) { return H * (H + 1); }
+// pairs stored before pair row i (H = RP / 2): sum over i' < i of (H - i'/2)
+__device__ __forceinline__ int pair_base(int i, int H) {
+  const int q = i >> 1;
+  return i * H - ((i & 1) ? q * q : q * (q - 1));
+}
+
 // Walks this warp's range of the stream (the MTTKRP kernel's nnz-balanced chunk ranges with one
 // lane group per warp) through a private TMA ring of kStages x kStageRecs records.  Lane l holds
 // columns 2l, 2l + 1.  For every record f(v, h, close, row, last) is called by the whole warp:
@@ -279,6 +289,9 @@ auto with_nmodes(int N, F && f) {
     default: return f(std::integral_constant<int, 8>{});
   }
 }
+
+// The compile-time rank tier of the pair-row kernels: R padded to 16, 32 or 64.
+int rank_tier(int R) { return R <= 16 ? 16 : (R <= 32 ? 32 : 64); }
 
 // Sets kernel k's dynamic shared memory to smem bytes and returns the grid of every CTA that can
 // be resident at that size, or 0 when k cannot run with it.
