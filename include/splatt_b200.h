@@ -751,6 +751,57 @@ int splatt_b200_cp_apr_pdnr_device(splatt_b200_tensor const * t, int ncolumns, i
                                    double * const * d_factors, double * lambda_out,
                                    double * history, int * iterations_out, void * stream);
 
+/* Parameters of CP-APR by PQNR beyond options[NITER] and options[TOLERANCE]. */
+typedef struct {
+  int    max_inner;      /* lockstep quasi-Newton iterations per mode, >= 1 (default 10) */
+  int    max_backtrack;  /* trial steps of the line search, 1..8 (default 8) */
+  int    lbfgs_mem;      /* L-BFGS pairs kept per row, 1..8 (default 3) */
+  double eps_active;     /* bound of the epsilon-active set, >= 0 (default 1e-8) */
+  double eps_div_zero;   /* floor of the model value in a division or a log, > 0 (default 1e-10) */
+} splatt_b200_pqnr_opts;
+
+/* Poisson CP decomposition by CP-APR with row-wise projected quasi-Newton steps (PQNR; Hansen,
+ * Plantenga & Kolda, Optim. Methods Softw. 2015).  Model, objective LL, start, outputs, outer
+ * loop, stop rule and the absence of a shift are those of splatt_b200_cp_apr_pdnr_device; only
+ * the direction differs, and it needs no Hessian.  In mode n every row i of B = A_n diag(lambda)
+ * starts from b = B[i,:] with no stored pair and level j = 0, and runs up to max_inner lockstep
+ * evaluations:
+ *   1. g = 1 - sum_x (v_x / max(m_x, eps)) Pi_x and kkt_i = max_r |min(b_r, g_r)|; if
+ *      kkt_i < TOLERANCE the row stops and keeps b.
+ *   2. After a previous step, if b is bitwise equal to b_prev (the last line search moved
+ *      nothing): j <- j + 1; at j = 3 the row stops; otherwise d <- 2^-max_backtrack d, so the
+ *      trial points continue the halving, and go to 5.
+ *   3. Otherwise j = 0, and after a previous step the pair s = b - b_prev, y = g - g_prev is
+ *      stored in a ring of lbfgs_mem pairs (the oldest dropped) if s.y > 0 and 1 / s.y is finite.
+ *   4. eps_i and the active set A are PDNR's; q = -g with q_A = 0; the L-BFGS two-loop recursion
+ *      over the stored pairs, newest to oldest, then a scaling by gamma = s.y / y.y of the newest
+ *      pair (1 when none is stored), then oldest to newest; d = q, then d_A = -g_A, and d = -g
+ *      when d is not finite.
+ *   5. b_prev = b, g_prev = g, and PDNR's line search along d: trial points
+ *      max(b + 2^-k d, 0), k = 0 .. max_backtrack-1, its Armijo and decrease tests and its
+ *      evaluation of the change; b stays unchanged when no trial point passes.
+ * Every scaling of d is a power of two, so the trial points do not depend on how the scalings
+ * are grouped.  A lockstep iteration in which no row gets a direction ends the mode without
+ * running the line search.
+ *   pqnr          NULL for the defaults (10, 8, 3, 1e-8, 1e-10).
+ *   d_factors[m], lambda_out, iterations_out: as splatt_b200_cp_apr_device.
+ *   history       NULL, or 4 doubles per outer iteration run: LL after it, the largest
+ *                 last-computed kkt_i over all rows and modes, the lockstep iterations run summed
+ *                 over the modes, and the line searches run (continuations included, whether or
+ *                 not a trial point passed) summed over rows and modes.
+ * On untiled streams lambda, the factors and the history's last three columns are bitwise
+ * reproducible from run to run; on leaf-tiled streams Phi and the line-search sums are added
+ * with atomics and may vary in the last bits.  Runs on t->device, enqueues on `stream`,
+ * synchronises it once per lockstep iteration (the count of rows with a direction) and once per
+ * outer iteration (the history).  VERBOSITY above NONE prints one line per outer iteration.
+ * Input rules: those of splatt_b200_cp_apr_device, and max_inner >= 1, 1 <= max_backtrack <= 8,
+ * 1 <= lbfgs_mem <= 8, eps_active >= 0 and eps > 0, all finite.  A violation returns
+ * SPLATT_ERROR_BADINPUT and the factors are left bit-identical. */
+int splatt_b200_cp_apr_pqnr_device(splatt_b200_tensor const * t, int ncolumns, int ldm,
+                                   double const * options, splatt_b200_pqnr_opts const * pqnr,
+                                   double * const * d_factors, double * lambda_out,
+                                   double * history, int * iterations_out, void * stream);
+
 /* TTMc, the kernel of Tucker: d_out = X_(mode) (kron_{m != mode} U_m), a dims[mode] x C_mode
  * row-major device matrix with leading dimension C_mode = prod_{m != mode} ranks[m], U_m =
  * columns [0, ranks[m]) of d_mats[m] (dims[m] x ldm, row-major).  Column order: the other modes

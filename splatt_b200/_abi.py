@@ -93,6 +93,11 @@ class PdnrOpts(C.Structure):
                 ("eps_active", C.c_double), ("eps_div_zero", C.c_double)]
 
 
+class PqnrOpts(C.Structure):
+    _fields_ = [("max_inner", C.c_int), ("max_backtrack", C.c_int), ("lbfgs_mem", C.c_int),
+                ("eps_active", C.c_double), ("eps_div_zero", C.c_double)]
+
+
 class TuckerOpts(C.Structure):
     _fields_ = [("max_power", C.c_int), ("svd_tol", C.c_double)]
 
@@ -119,7 +124,8 @@ EXPORTS = [
     "splatt_b200_cpd_nonneg_device", "splatt_b200_cpd_nonneg_device_f32",
     "splatt_b200_tensor_shard", "splatt_b200_mttkrp_multicast_sync",
     "splatt_b200_mttkrp_multicast_sync_columns", "splatt_b200_tensor_sse", "splatt_b200_tc_als_device",
-    "splatt_b200_cp_apr_device", "splatt_b200_cp_apr_pdnr_device", "splatt_b200_ttmc", "splatt_b200_tucker_hooi_device",
+    "splatt_b200_cp_apr_device", "splatt_b200_cp_apr_pdnr_device",
+    "splatt_b200_cp_apr_pqnr_device", "splatt_b200_ttmc", "splatt_b200_tucker_hooi_device",
     "splatt_b200_multi_env_devices", "splatt_b200_multi_create", "splatt_b200_multi_free",
     "splatt_b200_multi_info", "splatt_b200_multi_mttkrp_host", "splatt_b200_multi_cpd_als",
     "splatt_b200_multi_last_ms", "splatt_b200_build_count", "splatt_b200_cache_clear",
@@ -246,6 +252,10 @@ def load() -> C.CDLL:
     lib.splatt_b200_cp_apr_pdnr_device.restype = C.c_int
     lib.splatt_b200_cp_apr_pdnr_device.argtypes = [C.c_void_p, C.c_int, C.c_int,
                                                    C.POINTER(C.c_double), C.POINTER(PdnrOpts), vpp,
+                                                   val_p, val_p, C.POINTER(C.c_int), C.c_void_p]
+    lib.splatt_b200_cp_apr_pqnr_device.restype = C.c_int
+    lib.splatt_b200_cp_apr_pqnr_device.argtypes = [C.c_void_p, C.c_int, C.c_int,
+                                                   C.POINTER(C.c_double), C.POINTER(PqnrOpts), vpp,
                                                    val_p, val_p, C.POINTER(C.c_int), C.c_void_p]
     lib.splatt_b200_ttmc.restype = C.c_int
     lib.splatt_b200_ttmc.argtypes = [C.c_void_p, C.c_int, C.POINTER(C.c_int), C.c_int, vpp, val_p,

@@ -583,6 +583,36 @@ class Tensor:
         _check(rc, "splatt_b200_cp_apr_pdnr_device")
         return lam, [b[:, :rank] for b in bufs], hist[:its.value].copy(), its.value
 
+    def cp_apr_pqnr(self, rank: int, factors=None, *, niters: int = 50, tol: float = 1e-4,
+                    max_inner: int = 10, max_backtrack: int = 8, lbfgs_mem: int = 3,
+                    eps_active: float = 1e-8, eps: float = 1e-10, seed: int = 0,
+                    verbosity: int = 0, stream=None):
+        """Poisson CP decomposition by CP-APR with row-wise projected quasi-Newton steps
+        (PQNR, splatt_b200_cp_apr_pqnr_device): `cp_apr_pdnr` with the Newton direction replaced
+        by an L-BFGS direction from the last `lbfgs_mem` steps of each row, so no Hessian is
+        formed.  A row whose line search moves nothing continues the halving for up to two more
+        rounds, then stops.  Arguments, stop rule and return value as in `cp_apr_pdnr`; history
+        column 4 counts the line searches run."""
+        import torch
+        self._check_factors(factors, [rank] * self.nmodes, torch.float64, "CP-APR")
+        ldm = rank + (rank & 1)
+        bufs = self._start_factors(factors, [rank] * self.nmodes, ldm, torch.float64, seed,
+                                   lambda v, g: v.uniform_(0.0, 1.0, generator=g))
+        o = default_opts()
+        o[A.OPTION_NITER] = niters
+        o[A.OPTION_TOLERANCE] = tol
+        o[A.OPTION_VERBOSITY] = verbosity
+        po = A.PqnrOpts(max_inner, max_backtrack, lbfgs_mem, eps_active, eps)
+        s, ptrs = _launch_args(bufs, stream)
+        lam = np.zeros(rank)
+        hist = np.full((max(int(niters), 0), 4), np.nan)
+        its = C.c_int()
+        rc = self.lib.splatt_b200_cp_apr_pqnr_device(self.h, rank, ldm, _dptr(o), C.byref(po),
+                                                     ptrs, _dptr(lam), _dptr(hist), C.byref(its),
+                                                     C.c_void_p(s))
+        _check(rc, "splatt_b200_cp_apr_pqnr_device")
+        return lam, [b[:, :rank] for b in bufs], hist[:its.value].copy(), its.value
+
     def ttmc(self, mode: int, mats, out, ranks):
         """TTMc (splatt_b200_ttmc): out = X_(mode) times the Kronecker product of mats[m][:, :ranks[m]],
         m != mode, columns in mode order with the highest mode fastest.  mats: float64 CUDA tensors

@@ -675,6 +675,173 @@ __global__ void __launch_bounds__(kThreads) k_pdnr_kktmax(const double * __restr
   if ((threadIdx.x & 31) == 0) atomicMax(bits, static_cast<unsigned long long>(__double_as_longlong(m)));
 }
 
+// ---- PQNR: projected quasi-Newton (L-BFGS) on the rows ---------------------------------------------
+//
+// splatt_b200_cp_apr_pqnr_device.  The row problems of PDNR, with the direction from L-BFGS pairs
+// instead of the Hessian.  The gradient is 1 - Phi, and Phi is MU's, so one lockstep iteration
+// of mode n is k_apr_phi (+ k_apr_combine), k_pqnr_step for every row in state 1 (the pair
+// update and the direction), and -- when some row got a direction -- PDNR's k_pdnr_ladder
+// (+ k_apr_combine) and k_pdnr_accept.  The accept's damping goes to a scratch buffer PQNR never
+// reads.
+
+constexpr int kPqnrMaxMem = 8;          // the largest lbfgs_mem
+constexpr int kPqnrRounds = 3;          // continuation rounds before a row gives up
+
+// Per-row state of the quasi-Newton rows.  Pair slot k of row i is at S / Y + k * slot + i * ldm
+// (slot = max dims x ldm: a warp's row loads stay coalesced) and rho[k * rows_max + i].
+struct PqnrArgs {
+  const double * phi;          // rows x ldm: Phi at b
+  const double * B;            // rows x ldm: b
+  double *       D;            // rows x ldm: the direction (state 2)
+  double *       G;            // rows x ldm: g at b_prev, the accept's gradient
+  double *       Bp;           // rows x ldm: b_prev
+  double *       S;            // lbfgs_mem x slot
+  double *       Y;            // lbfgs_mem x slot
+  double *       rho;          // lbfgs_mem x rows_max: 1 / s.y
+  int *          head;         // rows: the ring slot the next pair goes to
+  int *          npairs;       // rows: pairs stored (<= lbfgs_mem)
+  int *          lev;          // rows: continuation level; -1 before the row's first step
+  int *          state;        // rows: 0 stopped, 1 to be evaluated, 2 has a direction
+  double *       kkt;          // rows: the last kkt
+  int *          count;        // rows that got a direction
+  unsigned long long rows, rows_max;
+  size_t         slot;
+  int            R, ldm, mem, max_backtrack;
+  double         tol, eps_active;
+};
+
+__device__ __forceinline__ double pqnr_wsum(double x) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) x += __shfl_xor_sync(0xffffffffu, x, o);
+  return x;
+}
+__device__ __forceinline__ double pqnr_dot(double2 a, double2 b) { return pqnr_wsum(fma(a.y, b.y, a.x * b.x)); }
+
+// One warp per row in state 1; lane l holds columns 2l, 2l + 1.  g = 1 - Phi and kkt; a row below
+// tol stops.  If the last line search left b bitwise unchanged, the level rises (the row stops at
+// kPqnrRounds) and d continues the halving (d <- 2^-max_backtrack d); otherwise the pair
+// (b - b_prev, g - g_prev) is stored when s.y > 0 and 1 / s.y is finite, and d comes from the
+// two-loop recursion on q = -g with q_A = 0, then d_A = -g_A (d = -g when not finite).  Stores
+// d, g and b as b_prev and g_prev, state 2, and adds the rows with a direction to *count.
+__global__ void __launch_bounds__(kThreads) k_pqnr_step(const PqnrArgs q) {
+  const int  warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const bool act  = 2 * lane < q.R;
+  const bool hasy = 2 * lane + 1 < q.R;
+  const int  mem  = q.mem;
+  int n = 0;
+  for (unsigned long long row = static_cast<unsigned long long>(blockIdx.x) * kWarps + warp; row < q.rows;
+       row += static_cast<unsigned long long>(gridDim.x) * kWarps) {
+    if (q.state[row] != 1) continue;
+    const size_t o = static_cast<size_t>(row) * q.ldm;
+    auto ld = [&](const double * base) {
+      double2 x = act ? reinterpret_cast<const double2 *>(base + o)[lane] : make_double2(0.0, 0.0);
+      if (!hasy) x.y = 0.0;
+      return x;
+    };
+    auto st = [&](double * base, double2 x) {
+      if (act) reinterpret_cast<double2 *>(base + o)[lane] = x;
+    };
+    const double2 b  = ld(q.B);
+    const double2 ph = ld(q.phi);
+    const double2 g  = make_double2(act ? 1.0 - ph.x : 0.0, hasy ? 1.0 - ph.y : 0.0);
+    double kkt = fmax(fabs(fmin(b.x, g.x)), fabs(fmin(b.y, g.y)));
+#pragma unroll
+    for (int s = 16; s > 0; s >>= 1) kkt = fmax(kkt, __shfl_xor_sync(0xffffffffu, kkt, s));
+    if (lane == 0) q.kkt[row] = kkt;
+    if (kkt < q.tol) {
+      if (lane == 0) q.state[row] = 0;
+      continue;
+    }
+    int lev = q.lev[row];
+    bool same = false;
+    double2 bp = make_double2(0.0, 0.0);
+    if (lev >= 0) {
+      bp = ld(q.Bp);
+      const bool eq = __double_as_longlong(b.x) == __double_as_longlong(bp.x) &&
+                      __double_as_longlong(b.y) == __double_as_longlong(bp.y);
+      same = __ballot_sync(0xffffffffu, !eq) == 0u;
+    }
+    double2 d;
+    if (same) {
+      if (++lev == kPqnrRounds) {
+        if (lane == 0) { q.lev[row] = lev; q.state[row] = 0; }
+        continue;
+      }
+      const double h = ldexp(1.0, -q.max_backtrack);
+      d = ld(q.D);
+      d = make_double2(h * d.x, h * d.y);
+    } else {
+      int head = q.head[row], np = q.npairs[row];
+      if (lev >= 0) {
+        const double2 gp  = ld(q.G);
+        const double2 s   = make_double2(b.x - bp.x, b.y - bp.y);
+        const double2 y   = make_double2(g.x - gp.x, g.y - gp.y);
+        const double  sty = pqnr_dot(s, y);
+        const double  r   = 1.0 / sty;
+        if (sty > 0.0 && isfinite(r)) {
+          const size_t k = static_cast<size_t>(head) * q.slot;
+          st(q.S + k, s);
+          st(q.Y + k, y);
+          if (lane == 0) q.rho[static_cast<size_t>(head) * q.rows_max + row] = r;
+          head = head + 1 == mem ? 0 : head + 1;
+          np   = min(np + 1, mem);
+        }
+      }
+      lev = 0;
+      const double tx = b.x - fmax(b.x - g.x, 0.0), ty = b.y - fmax(b.y - g.y, 0.0);
+      const double ei = fmin(q.eps_active, sqrt(pqnr_wsum(fma(ty, ty, tx * tx))));
+      const bool ax = act && b.x <= ei && g.x > 0.0;
+      const bool ay = hasy && b.y <= ei && g.y > 0.0;
+      double2 v = make_double2(ax ? 0.0 : -g.x, ay ? 0.0 : -g.y);
+      double alpha[kPqnrMaxMem];
+      double gamma = 1.0;
+#pragma unroll
+      for (int i = 0; i < kPqnrMaxMem; ++i) {  // newest to oldest
+        if (i < np) {
+          const int k = (head - 1 - i + 2 * mem) % mem;
+          const double2 sk = ld(q.S + static_cast<size_t>(k) * q.slot);
+          const double2 yk = ld(q.Y + static_cast<size_t>(k) * q.slot);
+          if (i == 0) gamma = pqnr_dot(sk, yk) / pqnr_dot(yk, yk);
+          alpha[i] = q.rho[static_cast<size_t>(k) * q.rows_max + row] * pqnr_dot(sk, v);
+          v = make_double2(fma(-alpha[i], yk.x, v.x), fma(-alpha[i], yk.y, v.y));
+        }
+      }
+      v = make_double2(gamma * v.x, gamma * v.y);
+#pragma unroll
+      for (int i = kPqnrMaxMem - 1; i >= 0; --i) {   // oldest to newest
+        if (i < np) {
+          const int k = (head - 1 - i + 2 * mem) % mem;
+          const double2 sk = ld(q.S + static_cast<size_t>(k) * q.slot);
+          const double2 yk = ld(q.Y + static_cast<size_t>(k) * q.slot);
+          const double beta = q.rho[static_cast<size_t>(k) * q.rows_max + row] * pqnr_dot(yk, v);
+          v = make_double2(fma(alpha[i] - beta, sk.x, v.x), fma(alpha[i] - beta, sk.y, v.y));
+        }
+      }
+      d = make_double2(ax ? -g.x : v.x, ay ? -g.y : v.y);
+      if (__ballot_sync(0xffffffffu, !(isfinite(d.x) && isfinite(d.y))) != 0u) d = make_double2(-g.x, -g.y);
+      if (lane == 0) { q.head[row] = head; q.npairs[row] = np; }
+    }
+    st(q.D, d);
+    st(q.G, g);
+    st(q.Bp, b);
+    if (lane == 0) { q.lev[row] = lev; q.state[row] = 2; }
+    ++n;
+  }
+  if (lane == 0 && n) atomicAdd(q.count, n);
+}
+
+// Every row of a mode: state 1, no pair, no step yet.
+__global__ void __launch_bounds__(kThreads) k_pqnr_init(int * __restrict__ state, int * __restrict__ head,
+                                                        int * __restrict__ npairs, int * __restrict__ lev,
+                                                        unsigned long long rows) {
+  for (unsigned long long i = blockIdx.x * static_cast<unsigned long long>(blockDim.x) + threadIdx.x; i < rows;
+       i += static_cast<unsigned long long>(gridDim.x) * blockDim.x) {
+    state[i] = 1;
+    head[i] = npairs[i] = 0;
+    lev[i] = -1;
+  }
+}
+
 #undef APR_FOR_ENTRIES
 
 // ---- host side ---------------------------------------------------------------------------------
@@ -707,9 +874,9 @@ struct AprBuffers {
 };
 
 
-// The extra device buffers of one PDNR run (B, the slots, lambda, the sums and the flags are
-// AprBuffers').
-struct PdnrBuffers : AprBuffers {
+// The extra device buffers of one run of a row method, PDNR or PQNR (B, the slots, lambda, the
+// sums and the flags are AprBuffers').
+struct RowBuffers : AprBuffers {
   double *   D = nullptr;                      // max dims x ldm: directions
   double *   G = nullptr;                      // max dims x ldm: gradients
   double *   lad = nullptr;                    // max dims x kPdnrTrials: ladder sums
@@ -717,10 +884,8 @@ struct PdnrBuffers : AprBuffers {
   double *   mu = nullptr;                     // max dims
   int *      state = nullptr;                  // max dims
   int *      count = nullptr;                  // one int: rows with a step
-  unsigned char * mark[SPB200_MAXN] = {nullptr};   // dims[m]: the row has a record
-  ~PdnrBuffers() {
+  ~RowBuffers() {
     cudaFree(D); cudaFree(G); cudaFree(lad); cudaFree(kkt_row); cudaFree(mu); cudaFree(state); cudaFree(count);
-    for (unsigned char * p : mark) cudaFree(p);
   }
 };
 
@@ -802,6 +967,341 @@ int apr_start(const splatt_b200_tensor * t, int R, int ldm, double * const * d_f
     fprintf(stderr, "SPLATT: %s failed (%s)\n", name, cudaGetErrorString(cudaGetLastError()));
     return SPLATT_ERROR_BADINPUT;
   }
+  return SPLATT_SUCCESS;
+}
+
+// ---- the row methods: one driver, PDNR's and PQNR's lockstep bodies ---------------------------
+
+// The options of both row methods.
+struct RowOpts {
+  int    max_inner, max_backtrack;
+  double eps_active, eps_div_zero;
+};
+
+// Reads the count of rows that got a step: a lockstep iteration's one synchronisation.
+bool read_count(const int * count, int & cnt, cudaStream_t s) {
+  return cudaGetLastError() == cudaSuccess &&
+         cudaMemcpyAsync(&cnt, count, sizeof(int), cudaMemcpyDeviceToHost, s) == cudaSuccess &&
+         cudaStreamSynchronize(s) == cudaSuccess;
+}
+
+// PDNR's lockstep iteration: the gradient and Hessian walk with the Newton directions
+// (k_pdnr_grad, k_pdnr_solve), the ladder and the accept.
+struct PdnrRows {
+  double mu0;
+  size_t P = 0;                                     // doubles of a gradient pack
+  WalkLaunch<PdnrArgs> gl[SPB200_MAXN], ll[SPB200_MAXN];
+  unsigned char * mark[SPB200_MAXN] = {nullptr};   // dims[m]: the row has a record
+  explicit PdnrRows(double mu0_) : mu0(mu0_) {}
+  ~PdnrRows() {
+    for (unsigned char * p : mark) cudaFree(p);
+  }
+
+  // per mode the gradient walk and the ladder walk; one pack buffer serves the largest need
+  // (boundary slots of either walk, or a pack per row on a leaf-tiled stream)
+  bool configure(const splatt_b200_tensor * t, int R, size_t & max_pack, unsigned long long & max_slot) {
+    const int RT = rank_tier(R), RP = R + (R & 1), H = RP / 2;
+    P = 2 * (size_t)H * (H + 1) + RP;
+    for (int m = 0; m < t->nmodes; ++m) {
+      const bool rows = t->streams[t->plan[m].stream].ktile_rows > 0;
+      auto lad = [rows](auto n) { return rows ? k_pdnr_ladder<n.value, true> : k_pdnr_ladder<n.value, false>; };
+      if (!gl[m].configure(with_nmodes(t->nmodes, [&](auto n) { return pdnr_grad_kernel<n.value>(RT, rows); }),
+                           pdnr_grad_smem(RT), rows) ||
+          !ll[m].configure(with_nmodes(t->nmodes, lad), tc_ring_bytes(), rows))
+        return false;
+      max_pack = std::max<size_t>({max_pack, (rows ? t->dims[m] : gl[m].nslots) * P, ll[m].nslots * kPdnrTrials});
+    }
+    max_slot = std::max({max_slots(gl, t->nmodes), max_slots(ll, t->nmodes), 1ull});
+    return true;
+  }
+  bool alloc(const splatt_b200_tensor * t, uint64_t, int) {
+    bool ok = true;
+    for (int m = 0; ok && m < t->nmodes; ++m)
+      ok = cudaMalloc(&mark[m], std::max<uint64_t>(t->dims[m], 1)) == cudaSuccess;
+    return ok;
+  }
+  bool reset(const splatt_b200_tensor * t, RowBuffers &, cudaStream_t s) {
+    bool ok = true;
+    for (int m = 0; ok && m < t->nmodes; ++m) ok = cudaMemsetAsync(mark[m], 0, t->dims[m], s) == cudaSuccess;
+    return ok;
+  }
+  void start_mode(int n, uint64_t rows, RowBuffers & b, PdnrArgs & p, cudaStream_t s) {
+    k_pdnr_init<<<elementwise_grid(rows, 1), kThreads, 0, s>>>(b.mu, b.state, rows, mu0);
+    spb200_count_launches(1);
+    p.w.slot_row = gl[n].rows ? nullptr : b.slot_row;
+    p.mark = mark[n];
+  }
+  bool lockstep(const FiberStream & fs, int n, uint64_t rows, const PdnrArgs & p, RowBuffers & b,
+                const RowOpts & o, cudaStream_t s, int & cnt) {
+    const WalkLaunch<PdnrArgs> & GL = gl[n];
+    const WalkLaunch<PdnrArgs> & LL = ll[n];
+    bool ok = true;
+    // gradient, Hessian and direction of every row still to be evaluated
+    if (GL.rows) ok = cudaMemsetAsync(b.packs, 0, rows * P * sizeof(double), s) == cudaSuccess;
+    if (ok && fs.nrec) ok = GL.launch(p, b.slot_row, s) == cudaSuccess;
+    ok = ok && launch_pdnr_solve(p, GL.nslots, rows, s) == cudaSuccess;
+    // the ladder's sums and the line search's decision
+    ok = ok && cudaMemsetAsync(b.lad, 0, rows * kPdnrTrials * sizeof(double), s) == cudaSuccess &&
+         cudaMemsetAsync(b.count, 0, sizeof(int), s) == cudaSuccess;
+    if (ok && fs.nrec) {
+      ok = LL.launch(p, b.slot_row, s) == cudaSuccess;
+      if (ok && !LL.rows) {
+        k_apr_combine<<<combine_grid(LL.nslots), kThreads, 0, s>>>(b.packs, b.slot_row, LL.nslots, kPdnrTrials,
+                                                                   kPdnrTrials, b.lad);
+        spb200_count_launches(1);
+      }
+    }
+    k_pdnr_accept<<<elementwise_grid(rows, 1), kThreads, 0, s>>>(b.B, b.D, b.G, b.lad, b.mu, b.state, rows,
+                                                                 p.w.R, p.w.ldm, o.max_backtrack, mu0, b.count);
+    spb200_count_launches(1);
+    return ok && read_count(b.count, cnt, s);
+  }
+};
+
+// PQNR's lockstep iteration: MU's Phi walk, k_pqnr_step, and -- only when some row got a
+// direction -- PDNR's ladder and accept.
+struct PqnrRows {
+  int mem;
+  WalkLaunch<TcArgs>   pl[SPB200_MAXN];
+  WalkLaunch<PdnrArgs> ll[SPB200_MAXN];
+  double * phi = nullptr;                           // max dims x ldm
+  double * Bp = nullptr;                            // max dims x ldm: b_prev
+  double * S = nullptr;                             // mem x max dims x ldm
+  double * Y = nullptr;                             // mem x max dims x ldm
+  double * rho = nullptr;                           // mem x max dims
+  int *    head = nullptr;                          // max dims (each)
+  int *    npairs = nullptr;
+  int *    lev = nullptr;
+  PqnrArgs q = {};
+  explicit PqnrRows(int mem_) : mem(mem_) {}
+  ~PqnrRows() {
+    cudaFree(phi); cudaFree(Bp); cudaFree(S); cudaFree(Y); cudaFree(rho); cudaFree(head); cudaFree(npairs);
+    cudaFree(lev);
+  }
+
+  // per mode the Phi walk and the ladder walk; one slot buffer serves both (a leaf-tiled stream
+  // adds its pieces into Phi and the ladder sums directly)
+  bool configure(const splatt_b200_tensor * t, int R, size_t & max_pack, unsigned long long & max_slot) {
+    const int RP = R + (R & 1);
+    for (int m = 0; m < t->nmodes; ++m) {
+      const bool rows = t->streams[t->plan[m].stream].ktile_rows > 0;
+      auto phik = [rows](auto n) { return rows ? k_apr_phi<n.value, true> : k_apr_phi<n.value, false>; };
+      auto lad = [rows](auto n) { return rows ? k_pdnr_ladder<n.value, true> : k_pdnr_ladder<n.value, false>; };
+      if (!pl[m].configure(with_nmodes(t->nmodes, phik), tc_ring_bytes(), rows) ||
+          !ll[m].configure(with_nmodes(t->nmodes, lad), tc_ring_bytes(), rows))
+        return false;
+      max_pack = std::max<size_t>({max_pack, pl[m].nslots * RP, ll[m].nslots * kPdnrTrials});
+    }
+    max_slot = std::max({max_slots(pl, t->nmodes), max_slots(ll, t->nmodes), 1ull});
+    return true;
+  }
+  bool alloc(const splatt_b200_tensor *, uint64_t max_dim, int ldm) {
+    const size_t slot = max_dim * ldm;
+    q.slot = slot;
+    q.rows_max = max_dim;
+    return cudaMalloc(&phi, slot * sizeof(double)) == cudaSuccess &&
+           cudaMalloc(&Bp, slot * sizeof(double)) == cudaSuccess &&
+           cudaMalloc(&S, mem * slot * sizeof(double)) == cudaSuccess &&
+           cudaMalloc(&Y, mem * slot * sizeof(double)) == cudaSuccess &&
+           cudaMalloc(&rho, mem * max_dim * sizeof(double)) == cudaSuccess &&
+           cudaMalloc(&head, max_dim * sizeof(int)) == cudaSuccess &&
+           cudaMalloc(&npairs, max_dim * sizeof(int)) == cudaSuccess &&
+           cudaMalloc(&lev, max_dim * sizeof(int)) == cudaSuccess;
+  }
+  // the accept's damping is never read; zero it once so it stays finite (mu0 = 0 keeps it 0)
+  bool reset(const splatt_b200_tensor *, RowBuffers & b, cudaStream_t s) {
+    return cudaMemsetAsync(b.mu, 0, q.rows_max * sizeof(double), s) == cudaSuccess;
+  }
+  void start_mode(int, uint64_t rows, RowBuffers & b, PdnrArgs & p, cudaStream_t s) {
+    k_pqnr_init<<<elementwise_grid(rows, 1), kThreads, 0, s>>>(b.state, head, npairs, lev, rows);
+    spb200_count_launches(1);
+    p.w.out = phi;
+    q.phi = phi; q.B = b.B; q.D = b.D; q.G = b.G; q.Bp = Bp; q.S = S; q.Y = Y; q.rho = rho;
+    q.head = head; q.npairs = npairs; q.lev = lev; q.state = b.state; q.kkt = b.kkt_row; q.count = b.count;
+    q.rows = rows; q.R = p.w.R; q.ldm = p.w.ldm; q.mem = mem;
+    q.tol = p.tol; q.eps_active = p.eps_active;
+  }
+  bool lockstep(const FiberStream & fs, int n, uint64_t rows, const PdnrArgs & p, RowBuffers & b,
+                const RowOpts & o, cudaStream_t s, int & cnt) {
+    const WalkLaunch<TcArgs> &   PL = pl[n];
+    const WalkLaunch<PdnrArgs> & LL = ll[n];
+    const int R = p.w.R, ldm = p.w.ldm;
+    // Phi at every row's b, then the pair update and the direction of every row still active
+    bool ok = cudaMemsetAsync(phi, 0, rows * ldm * sizeof(double), s) == cudaSuccess &&
+              cudaMemsetAsync(b.count, 0, sizeof(int), s) == cudaSuccess;
+    if (ok && fs.nrec) {
+      ok = PL.launch(p.w, b.slot_row, s) == cudaSuccess;
+      if (ok && !PL.rows) {
+        k_apr_combine<<<combine_grid(PL.nslots), kThreads, 0, s>>>(b.packs, b.slot_row, PL.nslots, R, ldm, phi);
+        spb200_count_launches(1);
+      }
+    }
+    q.max_backtrack = o.max_backtrack;
+    k_pqnr_step<<<combine_grid(rows), kThreads, 0, s>>>(q);
+    spb200_count_launches(1);
+    ok = ok && read_count(b.count, cnt, s);
+    if (!ok || !cnt) return ok;                     // no direction: the mode is done, no ladder
+    // the ladder's sums and the line search's decision
+    ok = cudaMemsetAsync(b.lad, 0, rows * kPdnrTrials * sizeof(double), s) == cudaSuccess;
+    if (ok && fs.nrec) {
+      ok = LL.launch(p, b.slot_row, s) == cudaSuccess;
+      if (ok && !LL.rows) {
+        k_apr_combine<<<combine_grid(LL.nslots), kThreads, 0, s>>>(b.packs, b.slot_row, LL.nslots, kPdnrTrials,
+                                                                   kPdnrTrials, b.lad);
+        spb200_count_launches(1);
+      }
+    }
+    k_pdnr_accept<<<elementwise_grid(rows, 1), kThreads, 0, s>>>(b.B, b.D, b.G, b.lad, b.mu, b.state, rows, R,
+                                                                 ldm, o.max_backtrack, 0.0, b.count);
+    spb200_count_launches(1);
+    return ok && cudaGetLastError() == cudaSuccess;
+  }
+};
+
+// The outer loop of both row methods (Body: PdnrRows or PqnrRows): the input rules (bad: the
+// body's own options violate them), the start, and per outer iteration and mode B = A_n diag(lambda),
+// up to max_inner lockstep iterations of the body, the largest kkt, the column sums and the
+// normalisation; the log-likelihood, lambda and the largest kkt are read back once per outer
+// iteration.
+template <class Body>
+int run_apr_rows(const char * name, const splatt_b200_tensor * t, int R, int ldm, const double * options,
+                 const RowOpts & o, bool bad, double * const * d_factors, double * lambda_out, double * history,
+                 int * iterations_out, void * stream, Body & body) {
+  const double tol = options ? options[SPLATT_OPTION_TOLERANCE] : 0.0;
+  const double niter = options ? options[SPLATT_OPTION_NITER] : 0.0;
+  auto nonneg = [](double x) { return std::isfinite(x) && x >= 0.0; };
+  auto positive = [](double x) { return std::isfinite(x) && x > 0.0; };
+  bad = bad || !root_streams_ok(t) || !options || !lambda_out ||
+        !factors_ok(t->nmodes, R, ldm, reinterpret_cast<const void * const *>(d_factors)) ||
+        o.max_inner < 1 || o.max_backtrack < 1 || o.max_backtrack > kPdnrTrials ||
+        !nonneg(o.eps_active) || !positive(o.eps_div_zero) || !nonneg(tol) ||
+        !(niter >= 0.0 && niter <= 2147483647.0);
+  if (bad) {
+    fprintf(stderr, "SPLATT: %s: bad arguments\n", name);
+    return SPLATT_ERROR_BADINPUT;
+  }
+  DeviceGuard g(t->device);
+  if (!g.ok) return SPLATT_ERROR_BADINPUT;
+  const int N = t->nmodes;
+  const int RP = R + (R & 1);
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const uint64_t niters = (uint64_t)niter;
+  const int verbosity = (int)options[SPLATT_OPTION_VERBOSITY];
+
+  uint64_t max_dim = 1;
+  for (int m = 0; m < N; ++m) max_dim = std::max<uint64_t>(max_dim, t->dims[m]);
+  size_t max_pack = 1;
+  unsigned long long max_slot = 1;
+  if (!body.configure(t, R, max_pack, max_slot)) {
+    fprintf(stderr, "SPLATT: %s: cannot configure the walks (%s)\n", name, cudaGetErrorString(cudaGetLastError()));
+    return SPLATT_ERROR_BADINPUT;
+  }
+  RowBuffers b;
+  bool ok = cudaMalloc(&b.B, max_dim * ldm * sizeof(double)) == cudaSuccess &&
+            cudaMalloc(&b.D, max_dim * ldm * sizeof(double)) == cudaSuccess &&
+            cudaMalloc(&b.G, max_dim * ldm * sizeof(double)) == cudaSuccess &&
+            cudaMalloc(&b.lad, max_dim * kPdnrTrials * sizeof(double)) == cudaSuccess &&
+            cudaMalloc(&b.kkt_row, max_dim * sizeof(double)) == cudaSuccess &&
+            cudaMalloc(&b.mu, max_dim * sizeof(double)) == cudaSuccess &&
+            cudaMalloc(&b.state, max_dim * sizeof(int)) == cudaSuccess &&
+            cudaMalloc(&b.count, sizeof(int)) == cudaSuccess &&
+            cudaMalloc(&b.packs, max_pack * sizeof(double)) == cudaSuccess &&
+            cudaMalloc(&b.slot_row, max_slot * sizeof(uint32_t)) == cudaSuccess &&
+            cudaMalloc(&b.lam, RP * sizeof(double)) == cudaSuccess &&
+            cudaMalloc(&b.sums, (size_t)N * RP * sizeof(double)) == cudaSuccess &&
+            cudaMalloc(&b.ll, sizeof(double)) == cudaSuccess &&
+            cudaMalloc(&b.kkt, sizeof(unsigned long long)) == cudaSuccess &&
+            cudaMalloc(&b.bad, sizeof(int)) == cudaSuccess &&
+            cudaMalloc(&b.colsum_part, kColsumCtas * 64 * sizeof(double)) == cudaSuccess &&
+            body.alloc(t, max_dim, ldm);
+  if (!ok) {
+    cudaGetLastError();
+    return SPLATT_ERROR_NOMEMORY;
+  }
+
+  std::vector<double> lam;
+  const int rc = apr_start(t, R, ldm, d_factors, b, lam, s, name);
+  if (rc != SPLATT_SUCCESS) return rc;
+  const FiberStream & fs0 = t->streams[0];
+  ok = cudaMemsetAsync(b.B, 0, max_dim * ldm * sizeof(double), s) == cudaSuccess && body.reset(t, b, s);
+
+  uint64_t its = 0;
+  auto t0 = std::chrono::steady_clock::now();
+  for (uint64_t it = 0; ok && it < niters; ++it) {
+    if (verbosity > SPLATT_VERBOSITY_NONE) t0 = std::chrono::steady_clock::now();
+    bool converged = true;
+    long long lockstep = 0, steps = 0;
+    ok = cudaMemsetAsync(b.kkt, 0, sizeof(unsigned long long), s) == cudaSuccess;
+    for (int n = 0; ok && n < N; ++n) {
+      const FiberStream & fs = t->streams[t->plan[n].stream];
+      const uint64_t rows = t->dims[n];
+      const unsigned eg = elementwise_grid(rows, R);
+      PdnrArgs p = {};
+      p.w = walk_args(fs, d_factors, ldm, R);
+      p.w.mats[0] = b.B;
+      p.w.eps = o.eps_div_zero;
+      p.w.packs = b.packs;
+      p.w.slot_row = b.slot_row;
+      p.D = b.D; p.G = b.G; p.lad = b.lad; p.kkt = b.kkt_row; p.mu = b.mu; p.state = b.state;
+      p.tol = tol; p.eps_active = o.eps_active;
+      // B = A_n diag(lambda) (no shift: A_n stands in for the unread Phi)
+      k_apr_scale<<<eg, kThreads, 0, s>>>(d_factors[n], d_factors[n], b.lam, b.B, rows, R, ldm, 0.0, 0.0, 0);
+      spb200_count_launches(1);
+      body.start_mode(n, rows, b, p, s);
+      for (int l = 0; ok && l < o.max_inner; ++l) {
+        int cnt = 0;
+        ok = body.lockstep(fs, n, rows, p, b, o, s, cnt);
+        if (!ok) break;
+        ++lockstep;
+        steps += cnt;
+        if (cnt && l == 0) converged = false;
+        if (!cnt) break;
+      }
+      if (!ok) break;
+      k_pdnr_kktmax<<<elementwise_grid(rows, 1), kThreads, 0, s>>>(b.kkt_row, rows, b.kkt);
+      spb200_count_launches(1);
+      launch_colsum(b.B, rows, R, ldm, b.colsum_part, b.lam, s);
+      k_apr_normalize<<<eg, kThreads, 0, s>>>(b.B, b.lam, d_factors[n], rows, R, ldm);
+      spb200_count_launches(1);
+    }
+    if (!ok) break;
+    // log-likelihood of the iteration's model, lambda and the largest kkt, read back once
+    double ll = 0.0, kkt_max = 0.0;
+    unsigned long long bits = 0;
+    ok = cudaMemsetAsync(b.ll, 0, sizeof(double), s) == cudaSuccess;
+    if (ok && fs0.nrec) {
+      TcArgs a = walk_args(fs0, d_factors, ldm, R);
+      a.lambda = b.lam; a.sse = b.ll; a.eps = o.eps_div_zero;
+      ok = launch_model_sum(with_nmodes(N, [](auto n) { return k_apr_ll<n.value>; }), a, s) == cudaSuccess;
+    }
+    ok = ok && cudaMemcpyAsync(&ll, b.ll, sizeof(double), cudaMemcpyDeviceToHost, s) == cudaSuccess &&
+         cudaMemcpyAsync(lam.data(), b.lam, RP * sizeof(double), cudaMemcpyDeviceToHost, s) == cudaSuccess &&
+         cudaMemcpyAsync(&bits, b.kkt, sizeof(bits), cudaMemcpyDeviceToHost, s) == cudaSuccess &&
+         cudaStreamSynchronize(s) == cudaSuccess;
+    if (!ok) break;
+    std::memcpy(&kkt_max, &bits, sizeof(kkt_max));
+    for (int r = 0; r < R; ++r) ll -= lam[r];
+    if (history) {
+      history[4 * it] = ll;
+      history[4 * it + 1] = kkt_max;
+      history[4 * it + 2] = (double)lockstep;
+      history[4 * it + 3] = (double)steps;
+    }
+    its = it + 1;
+    if (verbosity > SPLATT_VERBOSITY_NONE) {
+      const double sec = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
+      printf("  its = %3llu (%0.3fs)  log-likelihood = %0.10e  kkt = %0.3e  lockstep = %lld  steps = %lld\n",
+             (unsigned long long)its, sec, ll, kkt_max, lockstep, steps);
+    }
+    if (converged) break;
+  }
+  if (!ok) {
+    fprintf(stderr, "SPLATT: %s failed (%s)\n", name, cudaGetErrorString(cudaGetLastError()));
+    cudaStreamSynchronize(s);
+    return SPLATT_ERROR_BADINPUT;
+  }
+  std::copy(lam.begin(), lam.begin() + R, lambda_out);
+  if (iterations_out) *iterations_out = (int)its;
   return SPLATT_SUCCESS;
 }
 
@@ -968,180 +1468,22 @@ extern "C" int splatt_b200_cp_apr_pdnr_device(splatt_b200_tensor const * t, int 
                                               double const * options, splatt_b200_pdnr_opts const * pdnr,
                                               double * const * d_factors, double * lambda_out,
                                               double * history, int * iterations_out, void * stream) {
-  static const char * name = "splatt_b200_cp_apr_pdnr_device";
-  const int R = ncolumns;
   const splatt_b200_pdnr_opts o = pdnr ? *pdnr : splatt_b200_pdnr_opts{10, 8, 1e-5, 1e-8, 1e-10};
-  const double tol = options ? options[SPLATT_OPTION_TOLERANCE] : 0.0;
-  const double niter = options ? options[SPLATT_OPTION_NITER] : 0.0;
-  auto nonneg = [](double x) { return std::isfinite(x) && x >= 0.0; };
-  auto positive = [](double x) { return std::isfinite(x) && x > 0.0; };
-  bool bad = !root_streams_ok(t) || !options || !lambda_out ||
-             !factors_ok(t->nmodes, R, ldm, reinterpret_cast<const void * const *>(d_factors)) ||
-             o.max_inner < 1 || o.max_backtrack < 1 || o.max_backtrack > kPdnrTrials || !positive(o.mu0) ||
-             !nonneg(o.eps_active) || !positive(o.eps_div_zero) || !nonneg(tol) ||
-             !(niter >= 0.0 && niter <= 2147483647.0);
-  if (bad) {
-    fprintf(stderr, "SPLATT: %s: bad arguments\n", name);
-    return SPLATT_ERROR_BADINPUT;
-  }
-  DeviceGuard g(t->device);
-  if (!g.ok) return SPLATT_ERROR_BADINPUT;
-  const int N = t->nmodes;
-  const int RP = R + (R & 1), H = RP / 2;
-  const size_t P = 2 * (size_t)H * (H + 1) + RP;             // doubles of a gradient pack
-  const cudaStream_t s = static_cast<cudaStream_t>(stream);
-  const uint64_t niters = (uint64_t)niter;
-  const int verbosity = (int)options[SPLATT_OPTION_VERBOSITY];
+  PdnrRows body(o.mu0);
+  return run_apr_rows("splatt_b200_cp_apr_pdnr_device", t, ncolumns, ldm, options,
+                      RowOpts{o.max_inner, o.max_backtrack, o.eps_active, o.eps_div_zero},
+                      !(std::isfinite(o.mu0) && o.mu0 > 0.0), d_factors, lambda_out, history, iterations_out,
+                      stream, body);
+}
 
-  // per mode the gradient walk and the ladder walk; one pack buffer serves the largest need
-  // (boundary slots of either walk, or a pack per row on a leaf-tiled stream)
-  const int RT = rank_tier(R);
-  WalkLaunch<PdnrArgs> gl[SPB200_MAXN], ll[SPB200_MAXN];
-  uint64_t max_dim = 1;
-  size_t max_pack = 1;
-  for (int m = 0; m < N; ++m) {
-    const bool rows = t->streams[t->plan[m].stream].ktile_rows > 0;
-    auto lad = [rows](auto n) { return rows ? k_pdnr_ladder<n.value, true> : k_pdnr_ladder<n.value, false>; };
-    if (!gl[m].configure(with_nmodes(N, [&](auto n) { return pdnr_grad_kernel<n.value>(RT, rows); }),
-                         pdnr_grad_smem(RT), rows) ||
-        !ll[m].configure(with_nmodes(N, lad), tc_ring_bytes(), rows)) {
-      fprintf(stderr, "SPLATT: %s: cannot configure the walks (%s)\n", name, cudaGetErrorString(cudaGetLastError()));
-      return SPLATT_ERROR_BADINPUT;
-    }
-    max_dim = std::max<uint64_t>(max_dim, t->dims[m]);
-    max_pack = std::max<size_t>({max_pack, (rows ? t->dims[m] : gl[m].nslots) * P, ll[m].nslots * kPdnrTrials});
-  }
-  const unsigned long long max_slot = std::max({max_slots(gl, N), max_slots(ll, N), 1ull});
-  PdnrBuffers b;
-  bool ok = cudaMalloc(&b.B, max_dim * ldm * sizeof(double)) == cudaSuccess &&
-            cudaMalloc(&b.D, max_dim * ldm * sizeof(double)) == cudaSuccess &&
-            cudaMalloc(&b.G, max_dim * ldm * sizeof(double)) == cudaSuccess &&
-            cudaMalloc(&b.lad, max_dim * kPdnrTrials * sizeof(double)) == cudaSuccess &&
-            cudaMalloc(&b.kkt_row, max_dim * sizeof(double)) == cudaSuccess &&
-            cudaMalloc(&b.mu, max_dim * sizeof(double)) == cudaSuccess &&
-            cudaMalloc(&b.state, max_dim * sizeof(int)) == cudaSuccess &&
-            cudaMalloc(&b.count, sizeof(int)) == cudaSuccess &&
-            cudaMalloc(&b.packs, max_pack * sizeof(double)) == cudaSuccess &&
-            cudaMalloc(&b.slot_row, max_slot * sizeof(uint32_t)) == cudaSuccess &&
-            cudaMalloc(&b.lam, RP * sizeof(double)) == cudaSuccess &&
-            cudaMalloc(&b.sums, (size_t)N * RP * sizeof(double)) == cudaSuccess &&
-            cudaMalloc(&b.ll, sizeof(double)) == cudaSuccess &&
-            cudaMalloc(&b.kkt, sizeof(unsigned long long)) == cudaSuccess &&
-            cudaMalloc(&b.bad, sizeof(int)) == cudaSuccess &&
-            cudaMalloc(&b.colsum_part, kColsumCtas * 64 * sizeof(double)) == cudaSuccess;
-  for (int m = 0; ok && m < N; ++m)
-    ok = cudaMalloc(&b.mark[m], std::max<uint64_t>(t->dims[m], 1)) == cudaSuccess;
-  if (!ok) {
-    cudaGetLastError();
-    return SPLATT_ERROR_NOMEMORY;
-  }
-
-  std::vector<double> lam;
-  const int rc = apr_start(t, R, ldm, d_factors, b, lam, s, name);
-  if (rc != SPLATT_SUCCESS) return rc;
-  const FiberStream & fs0 = t->streams[0];
-  ok = cudaMemsetAsync(b.B, 0, max_dim * ldm * sizeof(double), s) == cudaSuccess;
-  for (int m = 0; ok && m < N; ++m) ok = cudaMemsetAsync(b.mark[m], 0, t->dims[m], s) == cudaSuccess;
-
-  uint64_t its = 0;
-  auto t0 = std::chrono::steady_clock::now();
-  for (uint64_t it = 0; ok && it < niters; ++it) {
-    if (verbosity > SPLATT_VERBOSITY_NONE) t0 = std::chrono::steady_clock::now();
-    bool converged = true;
-    long long lockstep = 0, steps = 0;
-    ok = cudaMemsetAsync(b.kkt, 0, sizeof(unsigned long long), s) == cudaSuccess;
-    for (int n = 0; ok && n < N; ++n) {
-      const FiberStream & fs = t->streams[t->plan[n].stream];
-      const WalkLaunch<PdnrArgs> & GL = gl[n];
-      const WalkLaunch<PdnrArgs> & LL = ll[n];
-      const uint64_t rows = t->dims[n];
-      const unsigned eg = elementwise_grid(rows, R);
-      // B = A_n diag(lambda) (no shift: A_n stands in for the unread Phi)
-      k_apr_scale<<<eg, kThreads, 0, s>>>(d_factors[n], d_factors[n], b.lam, b.B, rows, R, ldm, 0.0, 0.0, 0);
-      k_pdnr_init<<<elementwise_grid(rows, 1), kThreads, 0, s>>>(b.mu, b.state, rows, o.mu0);
-      spb200_count_launches(2);
-      PdnrArgs p = {};
-      p.w = walk_args(fs, d_factors, ldm, R);
-      p.w.mats[0] = b.B;
-      p.w.eps = o.eps_div_zero;
-      p.w.packs = b.packs;
-      p.w.slot_row = GL.rows ? nullptr : b.slot_row;
-      p.D = b.D; p.G = b.G; p.lad = b.lad; p.kkt = b.kkt_row; p.mu = b.mu; p.state = b.state;
-      p.mark = b.mark[n];
-      p.tol = tol; p.eps_active = o.eps_active;
-      for (int l = 0; ok && l < o.max_inner; ++l) {
-        // gradient, Hessian and direction of every row still to be evaluated
-        if (GL.rows) ok = cudaMemsetAsync(b.packs, 0, rows * P * sizeof(double), s) == cudaSuccess;
-        if (ok && fs.nrec) ok = GL.launch(p, b.slot_row, s) == cudaSuccess;
-        ok = ok && launch_pdnr_solve(p, GL.nslots, rows, s) == cudaSuccess;
-        // the ladder's sums and the line search's decision
-        ok = ok && cudaMemsetAsync(b.lad, 0, rows * kPdnrTrials * sizeof(double), s) == cudaSuccess &&
-             cudaMemsetAsync(b.count, 0, sizeof(int), s) == cudaSuccess;
-        if (ok && fs.nrec) {
-          ok = LL.launch(p, b.slot_row, s) == cudaSuccess;
-          if (ok && !LL.rows) {
-            k_apr_combine<<<combine_grid(LL.nslots), kThreads, 0, s>>>(b.packs, b.slot_row, LL.nslots, kPdnrTrials,
-                                                                       kPdnrTrials, b.lad);
-            spb200_count_launches(1);
-          }
-        }
-        k_pdnr_accept<<<elementwise_grid(rows, 1), kThreads, 0, s>>>(b.B, b.D, b.G, b.lad, b.mu, b.state, rows, R,
-                                                                     ldm, o.max_backtrack, o.mu0, b.count);
-        spb200_count_launches(1);
-        int cnt = 0;
-        ok = ok && cudaGetLastError() == cudaSuccess &&
-             cudaMemcpyAsync(&cnt, b.count, sizeof(int), cudaMemcpyDeviceToHost, s) == cudaSuccess &&
-             cudaStreamSynchronize(s) == cudaSuccess;
-        if (!ok) break;
-        ++lockstep;
-        steps += cnt;
-        if (cnt && l == 0) converged = false;
-        if (!cnt) break;
-      }
-      if (!ok) break;
-      k_pdnr_kktmax<<<elementwise_grid(rows, 1), kThreads, 0, s>>>(b.kkt_row, rows, b.kkt);
-      spb200_count_launches(1);
-      launch_colsum(b.B, rows, R, ldm, b.colsum_part, b.lam, s);
-      k_apr_normalize<<<eg, kThreads, 0, s>>>(b.B, b.lam, d_factors[n], rows, R, ldm);
-      spb200_count_launches(1);
-    }
-    if (!ok) break;
-    // log-likelihood of the iteration's model, lambda and the largest kkt, read back once
-    double ll = 0.0, kkt_max = 0.0;
-    unsigned long long bits = 0;
-    ok = cudaMemsetAsync(b.ll, 0, sizeof(double), s) == cudaSuccess;
-    if (ok && fs0.nrec) {
-      TcArgs a = walk_args(fs0, d_factors, ldm, R);
-      a.lambda = b.lam; a.sse = b.ll; a.eps = o.eps_div_zero;
-      ok = launch_model_sum(with_nmodes(N, [](auto n) { return k_apr_ll<n.value>; }), a, s) == cudaSuccess;
-    }
-    ok = ok && cudaMemcpyAsync(&ll, b.ll, sizeof(double), cudaMemcpyDeviceToHost, s) == cudaSuccess &&
-         cudaMemcpyAsync(lam.data(), b.lam, RP * sizeof(double), cudaMemcpyDeviceToHost, s) == cudaSuccess &&
-         cudaMemcpyAsync(&bits, b.kkt, sizeof(bits), cudaMemcpyDeviceToHost, s) == cudaSuccess &&
-         cudaStreamSynchronize(s) == cudaSuccess;
-    if (!ok) break;
-    std::memcpy(&kkt_max, &bits, sizeof(kkt_max));
-    for (int r = 0; r < R; ++r) ll -= lam[r];
-    if (history) {
-      history[4 * it] = ll;
-      history[4 * it + 1] = kkt_max;
-      history[4 * it + 2] = (double)lockstep;
-      history[4 * it + 3] = (double)steps;
-    }
-    its = it + 1;
-    if (verbosity > SPLATT_VERBOSITY_NONE) {
-      const double sec = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
-      printf("  its = %3llu (%0.3fs)  log-likelihood = %0.10e  kkt = %0.3e  lockstep = %lld  steps = %lld\n",
-             (unsigned long long)its, sec, ll, kkt_max, lockstep, steps);
-    }
-    if (converged) break;
-  }
-  if (!ok) {
-    fprintf(stderr, "SPLATT: %s failed (%s)\n", name, cudaGetErrorString(cudaGetLastError()));
-    cudaStreamSynchronize(s);
-    return SPLATT_ERROR_BADINPUT;
-  }
-  std::copy(lam.begin(), lam.begin() + R, lambda_out);
-  if (iterations_out) *iterations_out = (int)its;
-  return SPLATT_SUCCESS;
+extern "C" int splatt_b200_cp_apr_pqnr_device(splatt_b200_tensor const * t, int ncolumns, int ldm,
+                                              double const * options, splatt_b200_pqnr_opts const * pqnr,
+                                              double * const * d_factors, double * lambda_out,
+                                              double * history, int * iterations_out, void * stream) {
+  const splatt_b200_pqnr_opts o = pqnr ? *pqnr : splatt_b200_pqnr_opts{10, 8, 3, 1e-8, 1e-10};
+  PqnrRows body(o.lbfgs_mem);
+  return run_apr_rows("splatt_b200_cp_apr_pqnr_device", t, ncolumns, ldm, options,
+                      RowOpts{o.max_inner, o.max_backtrack, o.eps_active, o.eps_div_zero},
+                      o.lbfgs_mem < 1 || o.lbfgs_mem > kPqnrMaxMem, d_factors, lambda_out, history,
+                      iterations_out, stream, body);
 }
