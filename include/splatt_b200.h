@@ -643,6 +643,72 @@ int splatt_b200_tc_als_device(splatt_b200_tensor const * train,
                               double * const * d_factors, double * history,
                               int * iterations_out, void * stream);
 
+/* Parameters of completion by L-BFGS beyond options[NITER], [TOLERANCE] and [REGULARIZE]. */
+typedef struct {
+  int memory;   /* L-BFGS pairs kept, 0..32 (default 5); 0 = steepest descent with the exact line search */
+} splatt_b200_tc_lbfgs_opts;
+
+/* Tensor completion by whole-model L-BFGS with an exact line search (CP-WOPT; Acar, Dunlavy, Kolda
+ * & Morup, Chemometr. Intell. Lab. Syst. 2011).  Model and objective are those of
+ * splatt_b200_tc_als_device: x^ = sum_r prod_m U_m[i_m, r] and
+ *     L = sum_{x stored} (v_x - x^_x)^2 + reg * sum_m ||U_m||_F^2,   reg = options[REGULARIZE] >= 0,
+ * minimised over all factors at once.  U stands for the concatenation of the factors (columns
+ * [0, ncolumns) of every mode); g, d, s and y are vectors of that shape.  Iteration k, at U_k:
+ *   1. Gradient g_k = grad L(U_k), every mode's block at the same U_k:
+ *        G_m[i,:] = -2 sum_{x : i_m(x) = i} r_x h_x + 2 reg U_m[i,:],   r_x = v_x - x^_x,
+ *      h_x the Hadamard product of the other modes' rows (a row with no observations gets
+ *      2 reg U_m[i,:]).  From the second iteration on, the pair s = alpha_{k-1} d_{k-1},
+ *      y = g_k - g_{k-1} enters a ring of `memory` pairs (the oldest dropped) when s.y > 0.
+ *   2. Direction: if ||g_k||_2 = 0, alpha_k = 0 is recorded and the run stops.  Otherwise
+ *      d = -H g_k by the two-loop recursion over the stored pairs (newest to oldest, a scaling by
+ *      gamma = s.y / y.y of the newest pair, then oldest to newest); with no pair d = -g_k.  If
+ *      g.d is not negative the pairs are cleared and d = -g_k.
+ *   3. Exact line search: phi(a) = L(U_k + a d) = sum_{j=0}^{2N} c_j a^j, the data part from one
+ *      walk over the nonzeros and reg (||U||^2 + 2 a <U,d> + a^2 ||d||^2).  alpha_k minimises phi
+ *      over [0, B], B the Cauchy root bound of phi': the candidates are 0 and the real roots of
+ *      phi' in (0, B], and the smallest candidate with the least value is taken (alpha_k = 0 when
+ *      phi' is identically 0).  The decrease Delta = -sum_{j>=1} c_j alpha_k^j is evaluated from
+ *      the coefficients, not as a difference of two objectives.  If Delta <= 0 along a direction
+ *      from stored pairs, the pairs are cleared and the search is redone along -g_k in the same
+ *      iteration; if Delta <= 0 along -g_k, alpha_k = 0 is recorded, the factors stay unchanged
+ *      and the run stops.
+ *   4. U_{k+1} = U_k + alpha_k d.
+ * Stops after options[NITER] iterations, by the rules of steps 2 and 3, or, from the second
+ * iteration on, after an iteration with Delta / phi(0) < options[TOLERANCE].
+ *   lopts         NULL for the default (memory 5).
+ *   validate      may be NULL; else a tensor with train's nmodes and dims, on the same device,
+ *                 scored after every step.
+ *   d_factors[m]  dims[m] x ldm device matrices, in/out: the start on entry, U after the last step
+ *                 on return.  Columns [ncolumns, ldm) never feed a result and are never written.
+ *   history       NULL, or 5 doubles per iteration run: L after the step (phi(0) - Delta), the
+ *                 training RMSE after the step (from the data part of phi at alpha_k), the
+ *                 validation RMSE after the step (NaN without `validate`), alpha_k and ||g_k||_2.
+ *                 The first three columns are those of splatt_b200_tc_als_device.
+ *   iterations_out the number of iterations run (may be NULL).
+ * On untiled streams the factors, alpha and the first two history columns are bitwise
+ * reproducible from run to run (no sum that feeds them uses atomics); on leaf-tiled streams the
+ * gradient rows are added with atomics and may vary in the last bits.  Runs on train->device,
+ * enqueues on `stream` and synchronises it once per iteration (the line coefficients, ||g|| and
+ * g.d), twice in an iteration that retries along -g, and once at the end.  VERBOSITY above NONE
+ * prints one line per iteration.
+ * Input rules: those of splatt_b200_tc_als_device except that reg = 0 is allowed (reg finite and
+ * >= 0), and 0 <= memory <= 32.  A violation returns SPLATT_ERROR_BADINPUT before anything is
+ * enqueued, and the factors are left untouched. */
+int splatt_b200_tc_lbfgs_device(splatt_b200_tensor const * train, splatt_b200_tensor const * validate,
+                                int ncolumns, int ldm, double const * options,
+                                splatt_b200_tc_lbfgs_opts const * lopts,
+                                double * const * d_factors, double * history,
+                                int * iterations_out, void * stream);
+
+/* Host logic, no GPU needed: the exact line search of splatt_b200_tc_lbfgs_device.  For
+ * phi(a) = sum_{j=0}^{degree} c[j] a^j (0 <= degree <= 16, coefficients finite) writes the alpha
+ * of its step 3 and the decrease Delta = -sum_{j>=1} c[j] alpha^j.  The real roots of phi' in
+ * (0, B] are found where phi' changes sign (or vanishes exactly) between consecutive roots of
+ * phi'' -- found the same way one degree down -- and are bisected to full precision; a root where
+ * phi' touches 0 without changing sign cannot be a minimiser and is not returned.  Returns
+ * SPLATT_SUCCESS, or SPLATT_ERROR_BADINPUT (outputs untouched) on a bad argument. */
+int splatt_b200_poly_argmin(int degree, double const * c, double * alpha_out, double * decrease_out);
+
 /* Parameters of CP-APR beyond options[NITER] and options[TOLERANCE]. */
 typedef struct {
   int    max_inner;      /* inner (multiplicative-update) iterations per mode, >= 1 (default 10) */

@@ -98,6 +98,10 @@ class PqnrOpts(C.Structure):
                 ("eps_active", C.c_double), ("eps_div_zero", C.c_double)]
 
 
+class TcLbfgsOpts(C.Structure):
+    _fields_ = [("memory", C.c_int)]
+
+
 class TuckerOpts(C.Structure):
     _fields_ = [("max_power", C.c_int), ("svd_tol", C.c_double)]
 
@@ -124,6 +128,7 @@ EXPORTS = [
     "splatt_b200_cpd_nonneg_device", "splatt_b200_cpd_nonneg_device_f32",
     "splatt_b200_tensor_shard", "splatt_b200_mttkrp_multicast_sync",
     "splatt_b200_mttkrp_multicast_sync_columns", "splatt_b200_tensor_sse", "splatt_b200_tc_als_device",
+    "splatt_b200_tc_lbfgs_device", "splatt_b200_poly_argmin",
     "splatt_b200_cp_apr_device", "splatt_b200_cp_apr_pdnr_device",
     "splatt_b200_cp_apr_pqnr_device", "splatt_b200_ttmc", "splatt_b200_tucker_hooi_device",
     "splatt_b200_multi_env_devices", "splatt_b200_multi_create", "splatt_b200_multi_free",
@@ -245,6 +250,12 @@ def load() -> C.CDLL:
     lib.splatt_b200_tc_als_device.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int,
                                               C.POINTER(C.c_double), vpp, val_p,
                                               C.POINTER(C.c_int), C.c_void_p]
+    lib.splatt_b200_tc_lbfgs_device.restype = C.c_int
+    lib.splatt_b200_tc_lbfgs_device.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int,
+                                                C.POINTER(C.c_double), C.POINTER(TcLbfgsOpts), vpp,
+                                                val_p, C.POINTER(C.c_int), C.c_void_p]
+    lib.splatt_b200_poly_argmin.restype = C.c_int
+    lib.splatt_b200_poly_argmin.argtypes = [C.c_int, val_p, val_p, val_p]
     lib.splatt_b200_cp_apr_device.restype = C.c_int
     lib.splatt_b200_cp_apr_device.argtypes = [C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_double),
                                               C.POINTER(AprOpts), vpp, val_p, val_p,

@@ -510,6 +510,41 @@ class Tensor:
         _check(rc, "splatt_b200_tc_als_device")
         return hist[:its.value].copy(), [b[:, :rank] for b in bufs], its.value
 
+    def complete_lbfgs(self, rank: int, factors=None, *, validate: Optional["Tensor"] = None,
+                       reg: float, memory: int = 5, niters: int = 100, tol: float = 1e-6,
+                       seed: int = 0, verbosity: int = 0, stream=None):
+        """Tensor completion by whole-model L-BFGS with an exact line search
+        (splatt_b200_tc_lbfgs_device): the model and objective of `complete`, minimised over all
+        factors at once along L-BFGS directions from the last `memory` steps (0: steepest
+        descent), each step the exact minimiser of the objective along its direction.  reg >= 0.
+        Needs what `complete` needs; factors, seed and validate as in `complete`.  Stops after
+        `niters` iterations, when the gradient is zero or no decrease is found, or, from the
+        second iteration on, when the objective decreased by less than `tol` relative.
+        Returns (history: numpy float64 [iterations x 5] of (objective, training RMSE,
+        validation RMSE or NaN, step length, gradient norm), factors (CUDA views
+        dims[m] x rank), iterations)."""
+        import torch
+        self._check_factors(factors, [rank] * self.nmodes, torch.float64, "completion")
+        if validate is not None and not isinstance(validate, Tensor):
+            raise ValueError("validate must be a Tensor")
+        ldm = rank + (rank & 1)
+        bufs = self._start_factors(factors, [rank] * self.nmodes, ldm, torch.float64, seed,
+                                   lambda v, g: v.uniform_(0.0, 1.0, generator=g))
+        o = default_opts()
+        o[A.OPTION_NITER] = niters
+        o[A.OPTION_TOLERANCE] = tol
+        o[A.OPTION_VERBOSITY] = verbosity
+        o[A.OPTION_REGULARIZE] = reg
+        lo = A.TcLbfgsOpts(memory)
+        s, ptrs = _launch_args(bufs, stream)
+        hist = np.full((max(int(niters), 0), 5), np.nan)
+        its = C.c_int()
+        rc = self.lib.splatt_b200_tc_lbfgs_device(self.h, None if validate is None else validate.h,
+                                                  rank, ldm, _dptr(o), C.byref(lo), ptrs,
+                                                  _dptr(hist), C.byref(its), C.c_void_p(s))
+        _check(rc, "splatt_b200_tc_lbfgs_device")
+        return hist[:its.value].copy(), [b[:, :rank] for b in bufs], its.value
+
     def cp_apr(self, rank: int, factors=None, *, niters: int = 100, tol: float = 1e-4,
                max_inner: int = 10, kappa: float = 0.01, kappa_tol: float = 1e-10,
                eps: float = 1e-10, seed: int = 0, verbosity: int = 0, stream=None):

@@ -286,6 +286,13 @@ struct TcBuffers {
 };
 
 }  // namespace
+
+// launch_sse for the other completion solvers (tc_lbfgs.cu)
+cudaError_t tc_enqueue_sse(const FiberStream & fs, int R, int ldm, const double * const * d_mats_by_mode,
+                           const double * d_lambda, double * d_sse, cudaStream_t s) {
+  return launch_sse(fs, R, ldm, d_mats_by_mode, d_lambda, d_sse, s);
+}
+
 }  // namespace spb200
 
 using namespace spb200;
