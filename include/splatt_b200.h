@@ -938,6 +938,134 @@ int splatt_b200_tucker_hooi_device(splatt_b200_tensor const * t, int const * ran
                                    double * const * d_factors, double * core_out,
                                    double * history, int * iterations_out, void * stream);
 
+/* The nonzeros of a device tensor as coordinates, in the record order of its first stream
+ * (t->streams[0]: lexicographic in that stream's level order on an untiled stream; leaf-tiled
+ * streams regroup records inside ranges).  d_ind[m] (nnz_local uint32 each) and d_vals
+ * (nnz_local doubles) are caller-allocated DEVICE buffers; a shard writes its own nonzeros.
+ * One pass over the records, each 64-record chunk decoded from its descriptor, the records'
+ * close counts and the level ids up[l].  Works on every layout and tiling.  Runs on t->device,
+ * enqueues on `stream`; no host synchronisation.  Input rules: t non-NULL, every d_ind[m] and
+ * d_vals non-NULL; otherwise SPLATT_ERROR_BADINPUT and nothing is enqueued. */
+int splatt_b200_tensor_to_coo(splatt_b200_tensor const * t, uint32_t * const * d_ind, double * d_vals,
+                              void * stream);
+
+/* Losses of generalized CP (splatt_b200_gcp_*).  f(x, m), its derivative in m, and the values
+ * x a tensor may hold:
+ *   GAUSSIAN          (x - m)^2                                   2 (m - x)     finite
+ *   BERNOULLI_LOGIT   softplus(m) - x m,                          sigma(m) - x  0 or 1
+ *                     softplus(m) = max(m, 0) + log1p(exp(-|m|))
+ *   POISSON_LOG       exp(m) - x m                                exp(m) - x    finite, >= 0
+ * The stored-entry corrections f(x, m) - f(0, m) and df(x, m) - df(0, m) are evaluated as
+ * x^2 - 2 x m and -2 x (GAUSSIAN), -x m and -x (the others). */
+typedef enum {
+  SPLATT_B200_GCP_GAUSSIAN = 0,
+  SPLATT_B200_GCP_BERNOULLI_LOGIT = 1,
+  SPLATT_B200_GCP_POISSON_LOG = 2
+} splatt_b200_gcp_loss;
+
+/* Parameters of GCP-Adam beyond options[NITER], [TOLERANCE] and [VERBOSITY]. */
+typedef struct {
+  int      loss;         /* splatt_b200_gcp_loss (default BERNOULLI_LOGIT) */
+  int      grad_nnz;     /* p of every gradient sample: stored entries, >= 0 (default 65536) */
+  int      grad_zeros;   /* q of every gradient sample: uniform coordinates, >= 0 (default 65536) */
+  int      est_nnz;      /* p of the estimate sample, >= 0 (default 1048576) */
+  int      est_zeros;    /* q of the estimate sample, >= 0 (default 1048576) */
+  int      epoch_iters;  /* Adam steps per epoch, >= 1 (default 1000) */
+  double   lr;           /* learning rate of the first epoch, > 0 (default 1e-3) */
+  double   beta1;        /* first-moment decay, in [0, 1) (default 0.9) */
+  double   beta2;        /* second-moment decay, in [0, 1) (default 0.999) */
+  double   epsilon;      /* Adam's denominator floor, > 0 (default 1e-8) */
+  double   decay;        /* lr factor after a failed epoch, in (0, 1] (default 0.1) */
+  int      max_fails;    /* failed epochs tolerated, >= 0 (default 1) */
+  uint64_t seed;         /* key of every draw (default 0) */
+} splatt_b200_gcp_opts;
+
+/* Draws one sample set of GCP exactly as splatt_b200_gcp_device does.  Philox4x32-10 keyed by
+ * (seed & 0xffffffff, seed >> 32); draw j of step t_step under purpose P uses block b with counter
+ * (j, t_step & 0xffffffff, t_step >> 32, 4 P + b), and each 64-bit value is two consecutive words,
+ * the first one high.  Purposes: 0 gradient stored entries, 1 gradient coordinates, 2 estimate
+ * stored entries, 3 estimate coordinates (`estimate` 0 selects 0 and 1, else 2 and 3).
+ *   - sample j < p is a stored entry: the record position __umul64hi(v, nnz) in the record order
+ *     of splatt_b200_tensor_to_coo, v from block 0 words 0-1 with j the draw index;
+ *   - sample p + j (j < q) is a coordinate: mode n's index __umul64hi(v_n, dims[n]), v_n from
+ *     words 2 (n mod 2), 2 (n mod 2) + 1 of block n / 2, with j the draw index; its value is 0.
+ * d_ind[m] (p + q uint32 each) and d_vals (p + q doubles) are caller-allocated DEVICE buffers.
+ * The draws do not depend on the launch shape.  Decodes the tensor once into stream-ordered
+ * scratch of (4 N + 8) nnz bytes.  Runs on t->device and enqueues on `stream`; no host
+ * synchronisation.  Input rules: a whole tensor (shard_count <= 1); p, q >= 0, p + q >= 1 and
+ * p + q < 2^31; p = 0 when the tensor has no nonzero; every pointer non-NULL; otherwise
+ * SPLATT_ERROR_BADINPUT and nothing is enqueued. */
+int splatt_b200_gcp_sample(splatt_b200_tensor const * t, uint64_t seed, uint64_t t_step, int estimate,
+                           int p, int q, uint32_t * const * d_ind, double * d_vals, void * stream);
+
+/* The kernel primitive of GCP on an explicit sample of p + q coordinates (d_ind[m], p + q uint32
+ * each, on the device): samples 0 .. p-1 are stored entries with values d_vals[0 .. p-1] and weight
+ * w_nz, samples p .. p+q-1 are coordinates (value 0) with weight w_z.  With m_s the model
+ * sum_r prod_n U_n[i_n, r] at sample s,
+ *     value = sum_{s < p} w_nz (f(x_s, m_s) - f(0, m_s)) + sum_{s >= p} w_z f(0, m_s),
+ *     G_n[i, :] = sum_{s : i_n(s) = i} y_s prod_{k != n} U_k[i_k(s), :],
+ *     y_s = w_nz (df(x_s, m_s) - df(0, m_s)) (s < p),  w_z df(0, m_s) (s >= p).
+ *   d_factors[m]  dims[m] x ldm device matrices; columns [ncolumns, ldm) are never read.
+ *   d_grads       NULL (value only), or dims[m] x ldm device matrices: columns [0, ncolumns) are
+ *                 zeroed and then accumulated into, the other columns never written.
+ *   value_out     NULL (no value, no host synchronisation), or one HOST double.
+ * The value is summed in a fixed order (per warp in sample order, then warps, then CTAs in order)
+ * and is bitwise reproducible; the gradient rows are added with red.add.f64 atomics and are not.
+ * Runs on t->device and enqueues on `stream`; synchronises it once when value_out is given.
+ * Input rules: loss one of splatt_b200_gcp_loss; 1 <= ncolumns <= 64; ldm even and >= ncolumns;
+ * every d_factors[m] (and d_grads[m]) non-NULL and 16-byte aligned; p, q >= 0, p + q < 2^31; w_nz
+ * and w_z finite; d_vals non-NULL when p > 0.  Indices must lie inside dims (not checked).  A
+ * violation returns SPLATT_ERROR_BADINPUT and nothing is enqueued. */
+int splatt_b200_gcp_sampled(splatt_b200_tensor const * t, int loss, int p, int q, double w_nz,
+                            double w_z, uint32_t const * const * d_ind, double const * d_vals,
+                            int ncolumns, int ldm, double const * const * d_factors,
+                            double * const * d_grads, double * value_out, void * stream);
+
+/* Generalized CP decomposition (GCP; Hong, Kolda & Duersch, SIAM Rev. 2020) by sampled gradients
+ * and Adam (GCP-Adam; Kolda & Hong, SIMODS 2020, Alg. 5.1).  The model m_x = sum_r prod_n
+ * U_n[i_n, r] (no lambda) is fitted to every coordinate, unstored ones being x = 0:
+ *     F(U) = sum_{all coordinates} f(0, m) + sum_{stored x} (f(x_v, m_x) - f(0, m_x)),
+ * f the loss of gopts->loss; duplicate coordinates count separately.  With nnz the stored entries
+ * and P = prod dims[n] (in fp64), a sample of p stored entries and q coordinates
+ * (splatt_b200_gcp_sample) weighted w_nz = nnz / p and w_z = P / q (0 when p or q is 0) gives
+ * unbiased estimates of F and grad F (splatt_b200_gcp_sampled).
+ *   Steps.  The global step count t starts at 0.  A step draws the gradient sample of step t,
+ *     forms every mode's gradient G at the same U, and applies Adam to columns [0, ncolumns):
+ *       M = b1 M + (1 - b1) G,  V = b2 V + (1 - b2) G^2,
+ *       U -= lr (M / (1 - b1^(t+1))) / (sqrt(V / (1 - b2^(t+1))) + eps);
+ *     then t = t + 1.  M and V start at 0.
+ *   Epochs.  An epoch is epoch_iters steps; at its end F is estimated on one estimate sample
+ *     drawn once per call (t_step = 0, purposes 2 and 3).  The epoch is accepted if the estimate
+ *     is finite and <= the last accepted estimate (the start's estimate at first).  Otherwise it
+ *     fails: U, M, V and t return bitwise to their values at the epoch's start and lr *= decay.
+ *   Stops after options[NITER] epochs, after more than max_fails failed epochs, or after an
+ *     accepted epoch whose relative decrease (prev - est) / |prev| is < options[TOLERANCE] (a
+ *     previous estimate of 0 counts as no decrease).
+ *   gopts         NULL for the defaults (BERNOULLI_LOGIT, 65536, 65536, 1048576, 1048576, 1000,
+ *                 1e-3, 0.9, 0.999, 1e-8, 0.1, 1, 0).
+ *   d_factors[m]  dims[m] x ldm device matrices, in/out: the start on entry, U after the last
+ *                 accepted (or the start, when none) epoch's end on return.  Columns
+ *                 [ncolumns, ldm) never feed a result and are never written.
+ *   history       NULL, or 3 doubles per epoch run: the estimate at its end, the lr it used, and
+ *                 1 if it was accepted, else 0.
+ *   f_start_out   NULL, or one HOST double: the estimate at the start.
+ *   epochs_out    the number of epochs run (may be NULL).
+ * The gradients are summed with atomics, so U is not bitwise reproducible from run to run; given
+ * the gradient, the estimate and the Adam update are elementwise and deterministic.  The stored
+ * entries are decoded once per call into (4 N + 8) nnz bytes of device memory beside the sample
+ * buffers.  Runs on t->device, enqueues on `stream` and synchronises it once per epoch (the
+ * estimate) and a bounded number of times at the start (the value check, the start's estimate);
+ * never within an epoch.  VERBOSITY above NONE prints one line per epoch.
+ * Input rules: a whole tensor (shard_count <= 1) of 2..8 modes, any layout; 1 <= ncolumns <= 64;
+ * ldm even and >= ncolumns; every d_factors[m] 16-byte aligned; every tensor value allowed by
+ * the loss (checked on the device); p, q >= 0 and 1 <= p + q < 2^31 for both samples, p = 0 when
+ * the tensor has no nonzero; epoch_iters >= 1; lr > 0, 0 <= beta1, beta2 < 1, epsilon > 0,
+ * 0 < decay <= 1, all finite; max_fails >= 0; TOLERANCE finite; 0 <= NITER < 2^31.  A violation
+ * returns SPLATT_ERROR_BADINPUT, and the factors are left bit-identical. */
+int splatt_b200_gcp_device(splatt_b200_tensor const * t, int ncolumns, int ldm, double const * options,
+                           splatt_b200_gcp_opts const * gopts, double * const * d_factors,
+                           double * history, double * f_start_out, int * epochs_out, void * stream);
+
 /* Measurement aid: a pure gather kernel with the MTTKRP's access pattern (whole
  * fp64 rows of a rows x ldm matrix at d_idx[0..nidx), 128-bit loads, eight rows in
  * flight per lane group, no arithmetic).  bench.py times it to report a MEASURED

@@ -102,6 +102,19 @@ class TcLbfgsOpts(C.Structure):
     _fields_ = [("memory", C.c_int)]
 
 
+class GcpOpts(C.Structure):
+    _fields_ = [("loss", C.c_int), ("grad_nnz", C.c_int), ("grad_zeros", C.c_int),
+                ("est_nnz", C.c_int), ("est_zeros", C.c_int), ("epoch_iters", C.c_int),
+                ("lr", C.c_double), ("beta1", C.c_double), ("beta2", C.c_double),
+                ("epsilon", C.c_double), ("decay", C.c_double), ("max_fails", C.c_int),
+                ("seed", C.c_uint64)]
+
+
+GCP_GAUSSIAN, GCP_BERNOULLI_LOGIT, GCP_POISSON_LOG = 0, 1, 2
+GCP_LOSSES = {"gaussian": GCP_GAUSSIAN, "bernoulli-logit": GCP_BERNOULLI_LOGIT,
+              "poisson-log": GCP_POISSON_LOG}
+
+
 class TuckerOpts(C.Structure):
     _fields_ = [("max_power", C.c_int), ("svd_tol", C.c_double)]
 
@@ -131,6 +144,8 @@ EXPORTS = [
     "splatt_b200_tc_lbfgs_device", "splatt_b200_poly_argmin",
     "splatt_b200_cp_apr_device", "splatt_b200_cp_apr_pdnr_device",
     "splatt_b200_cp_apr_pqnr_device", "splatt_b200_ttmc", "splatt_b200_tucker_hooi_device",
+    "splatt_b200_tensor_to_coo", "splatt_b200_gcp_sample", "splatt_b200_gcp_sampled",
+    "splatt_b200_gcp_device",
     "splatt_b200_multi_env_devices", "splatt_b200_multi_create", "splatt_b200_multi_free",
     "splatt_b200_multi_info", "splatt_b200_multi_mttkrp_host", "splatt_b200_multi_cpd_als",
     "splatt_b200_multi_last_ms", "splatt_b200_build_count", "splatt_b200_cache_clear",
@@ -275,6 +290,19 @@ def load() -> C.CDLL:
     lib.splatt_b200_tucker_hooi_device.argtypes = [C.c_void_p, C.POINTER(C.c_int), C.c_int,
                                                    C.POINTER(C.c_double), C.POINTER(TuckerOpts), vpp,
                                                    val_p, val_p, C.POINTER(C.c_int), C.c_void_p]
+    lib.splatt_b200_tensor_to_coo.restype = C.c_int
+    lib.splatt_b200_tensor_to_coo.argtypes = [C.c_void_p, u32pp, val_p, C.c_void_p]
+    lib.splatt_b200_gcp_sample.restype = C.c_int
+    lib.splatt_b200_gcp_sample.argtypes = [C.c_void_p, C.c_uint64, C.c_uint64, C.c_int, C.c_int,
+                                           C.c_int, u32pp, val_p, C.c_void_p]
+    lib.splatt_b200_gcp_sampled.restype = C.c_int
+    lib.splatt_b200_gcp_sampled.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_double,
+                                            C.c_double, u32pp, val_p, C.c_int, C.c_int, vpp, vpp,
+                                            C.POINTER(C.c_double), C.c_void_p]
+    lib.splatt_b200_gcp_device.restype = C.c_int
+    lib.splatt_b200_gcp_device.argtypes = [C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_double),
+                                           C.POINTER(GcpOpts), vpp, val_p, val_p,
+                                           C.POINTER(C.c_int), C.c_void_p]
     lib.splatt_b200_csf_to_coo.restype = C.c_int
     lib.splatt_b200_csf_to_coo.argtypes = [csf_p, u32pp, val_p]
     lib.splatt_b200_gather_probe.restype = C.c_int

@@ -212,6 +212,15 @@ def _launch_args(bufs, stream, ptr_t=A.val_p):
     return s, (ptr_t * len(bufs))(*[C.cast(C.c_void_p(b.data_ptr()), ptr_t) for b in bufs])
 
 
+def _u32_ptrs(bufs):
+    """ctypes array of uint32 pointers to int32/uint32 CUDA tensors (indices below 2^31)."""
+    for b in bufs:
+        if b.element_size() != 4 or not b.is_contiguous():
+            raise ValueError("index buffers must be contiguous 32-bit integer tensors")
+    return (C.POINTER(C.c_uint32) * len(bufs))(*[C.cast(C.c_void_p(b.data_ptr()), C.POINTER(C.c_uint32))
+                                                  for b in bufs])
+
+
 class Tensor:
     """Device-resident sparse tensor (splatt_b200_tensor): per-mode fiber streams in HBM."""
 
@@ -728,6 +737,125 @@ class Tensor:
         _check(rc, "splatt_b200_tucker_hooi_device")
         return (core.reshape(ranks), [b[:, :r] for b, r in zip(bufs, ranks)], hist[:its.value].copy(),
                 its.value)
+
+    def to_coo(self, stream=None):
+        """This tensor's (local) nonzeros as coordinates in the record order of its first stream
+        (splatt_b200_tensor_to_coo).  Returns (inds: one int32 CUDA tensor per mode, vals: a
+        float64 CUDA tensor), on the current device."""
+        import torch
+        dev = torch.device("cuda", torch.cuda.current_device())
+        inds = [torch.empty(self.nnz_local, dtype=torch.int32, device=dev) for _ in range(self.nmodes)]
+        vals = torch.empty(self.nnz_local, dtype=torch.float64, device=dev)
+        s = torch.cuda.current_stream(dev).cuda_stream if stream is None else stream
+        rc = self.lib.splatt_b200_tensor_to_coo(self.h, _u32_ptrs(inds), C.cast(C.c_void_p(vals.data_ptr()), A.val_p),
+                                                C.c_void_p(s))
+        _check(rc, "splatt_b200_tensor_to_coo")
+        return inds, vals
+
+    def gcp_sample(self, seed: int, step: int, p: int, q: int, estimate: bool = False, stream=None):
+        """One GCP sample set as the driver draws it (splatt_b200_gcp_sample): p stored entries
+        drawn with replacement, then q uniform coordinates with value 0, from the Philox stream of
+        `seed` at step `step` (estimate: the estimate sample's purposes).  Returns (inds: one int32
+        CUDA tensor of p + q per mode, vals: float64 CUDA tensor of p + q)."""
+        import torch
+        dev = torch.device("cuda", torch.cuda.current_device())
+        n = max(int(p) + int(q), 0)
+        inds = [torch.empty(n, dtype=torch.int32, device=dev) for _ in range(self.nmodes)]
+        vals = torch.empty(n, dtype=torch.float64, device=dev)
+        s = torch.cuda.current_stream(dev).cuda_stream if stream is None else stream
+        rc = self.lib.splatt_b200_gcp_sample(self.h, int(seed), int(step), int(bool(estimate)), int(p), int(q),
+                                             _u32_ptrs(inds), C.cast(C.c_void_p(vals.data_ptr()), A.val_p),
+                                             C.c_void_p(s))
+        _check(rc, "splatt_b200_gcp_sample")
+        return inds, vals
+
+    def gcp_sampled(self, loss, inds, vals, p: int, q: int, w_nz: float, w_z: float, factors, *,
+                    rank: Optional[int] = None, grads=True, stream=None):
+        """The GCP kernel primitive (splatt_b200_gcp_sampled) on an explicit sample: inds (one
+        int32 CUDA tensor of >= p + q per mode) and vals (float64, the first p are read) with
+        samples 0..p-1 stored entries of weight w_nz and p..p+q-1 coordinates of weight w_z.
+        factors: float64 CUDA tensors (dims[m] x >= rank), used in place when they share one
+        even, 16-byte-aligned row stride, else copied into padded buffers.  grads: True (new
+        buffers), False (value only), or a list of float64 CUDA tensors laid out like the
+        factors, whose first `rank` columns are overwritten.  Returns (value, grads or None)."""
+        import torch
+        loss = A.GCP_LOSSES[loss] if isinstance(loss, str) else int(loss)
+        R = factors[0].shape[1] if rank is None else int(rank)
+        dev = torch.device("cuda", torch.cuda.current_device())
+        ldm = factors[0].stride(0)
+        direct = (len(factors) == self.nmodes and ldm % 2 == 0 and ldm >= R and
+                  all(f.dtype == torch.float64 and f.device == dev and f.stride(1) == 1 and f.stride(0) == ldm
+                      and f.data_ptr() % 16 == 0 and tuple(f.shape[:1]) == (self.dims[m],) and f.shape[1] >= R
+                      for m, f in enumerate(factors)))
+        if not direct:
+            self._check_factors([f[:, :R] for f in factors], [R] * self.nmodes, torch.float64, "GCP")
+            ldm = R + (R & 1)
+            factors = self._start_factors([f[:, :R] for f in factors], [R] * self.nmodes, ldm, torch.float64)
+        if grads is True:
+            gbufs = [torch.zeros((d, ldm), dtype=torch.float64, device=dev) for d in self.dims]
+        elif grads:
+            gbufs = list(grads)
+            if any(g.stride(0) != ldm or g.stride(1) != 1 or g.dtype != torch.float64 for g in gbufs):
+                raise ValueError("grads must be float64 CUDA tensors with the factors' row stride")
+        else:
+            gbufs = None
+        if stream is not None:
+            torch.cuda.current_stream(dev).synchronize()      # the buffers were filled there
+        s = torch.cuda.current_stream(dev).cuda_stream if stream is None else stream
+        fp = (A.val_p * self.nmodes)(*[C.cast(C.c_void_p(f.data_ptr()), A.val_p) for f in factors])
+        gp = None if gbufs is None else (A.val_p * self.nmodes)(*[C.cast(C.c_void_p(g.data_ptr()), A.val_p)
+                                                                  for g in gbufs])
+        out = C.c_double()
+        rc = self.lib.splatt_b200_gcp_sampled(self.h, loss, int(p), int(q), float(w_nz), float(w_z),
+                                              _u32_ptrs(inds), C.cast(C.c_void_p(vals.data_ptr()), A.val_p),
+                                              R, ldm, fp, gp, C.byref(out), C.c_void_p(s))
+        _check(rc, "splatt_b200_gcp_sampled")
+        return out.value, None if gbufs is None else [g[:, :R] for g in gbufs]
+
+    def gcp(self, rank: int, loss="bernoulli-logit", factors=None, *, niters: int = 50,
+            tol: float = 1e-4, grad_samples=(1 << 16, 1 << 16), est_samples=(1 << 20, 1 << 20),
+            epoch_iters: int = 1000, lr: float = 1e-3, beta1: float = 0.9, beta2: float = 0.999,
+            epsilon: float = 1e-8, decay: float = 0.1, max_fails: int = 1, seed: int = 0,
+            verbosity: int = 0, stream=None):
+        """Generalized CP decomposition by sampled gradients and Adam (GCP-Adam,
+        splatt_b200_gcp_device): fits sum_r prod_m U_m[i_m, r] to every coordinate of this
+        tensor (unstored ones being 0) under `loss` ("gaussian", "bernoulli-logit" or
+        "poisson-log").  Each step draws grad_samples = (p stored entries, q coordinates) and
+        applies one Adam update; an epoch of `epoch_iters` steps is scored on one fixed sample of
+        est_samples and accepted if the estimate did not rise, else undone with lr *= decay.
+        Stops after `niters` epochs, more than `max_fails` failed epochs, or an accepted epoch
+        that decreased the estimate by less than `tol` relative.  Needs a whole tensor on the
+        current CUDA device, values allowed by the loss, and 1 <= rank <= 64.  float64 only.
+
+        factors: list of float64 CUDA tensors (dims[m] x rank), the start; copied into padded
+        buffers, never written.  None: N(0, 1) R^(-1/(2N)) entries from a torch.Generator on the
+        current device seeded with `seed` (so the model starts with unit variance); `seed` also
+        keys every sample.
+        Returns (factors (CUDA views dims[m] x rank), history (numpy float64 [epochs x 3] of
+        (estimate, lr used, accepted 1/0)), epochs, f_start (the estimate at the start))."""
+        import torch
+        self._check_factors(factors, [rank] * self.nmodes, torch.float64, "GCP")
+        if loss not in A.GCP_LOSSES:
+            raise ValueError(f"loss must be one of {sorted(A.GCP_LOSSES)}, not {loss!r}")
+        ldm = rank + (rank & 1)
+        scale = float(rank) ** (-1.0 / (2 * self.nmodes)) if rank > 0 else 1.0
+        bufs = self._start_factors(factors, [rank] * self.nmodes, ldm, torch.float64, seed,
+                                   lambda v, g: v.normal_(0.0, 1.0, generator=g).mul_(scale))
+        o = default_opts()
+        o[A.OPTION_NITER] = niters
+        o[A.OPTION_TOLERANCE] = tol
+        o[A.OPTION_VERBOSITY] = verbosity
+        go = A.GcpOpts(A.GCP_LOSSES[loss], int(grad_samples[0]), int(grad_samples[1]), int(est_samples[0]),
+                       int(est_samples[1]), int(epoch_iters), lr, beta1, beta2, epsilon, decay,
+                       int(max_fails), int(seed) & 0xFFFFFFFFFFFFFFFF)
+        s, ptrs = _launch_args(bufs, stream)
+        hist = np.full((max(int(niters), 0), 3), np.nan)
+        f0 = C.c_double(np.nan)
+        its = C.c_int()
+        rc = self.lib.splatt_b200_gcp_device(self.h, rank, ldm, _dptr(o), C.byref(go), ptrs, _dptr(hist),
+                                             C.byref(f0), C.byref(its), C.c_void_p(s))
+        _check(rc, "splatt_b200_gcp_device")
+        return [b[:, :rank] for b in bufs], hist[:its.value].copy(), its.value, f0.value
 
     def shard(self, rank: int, count: int, device: int = -1) -> "Tensor":
         """Cut shard `rank` of `count` out of this (whole) tensor onto `device`
